@@ -53,6 +53,7 @@ ALGO_BYTES = {"pmc": 1676, "epmc": 6208, "epmc_flat": 4672, "sepmc": 9576}
 OBS_W = {"pmc": 207, "epmc": 916, "sepmc": 965}
 ROBOTS_PER_ENV = {"pmc": 1, "epmc": 1, "sepmc": 2}
 ELEMENT = [3]
+DUMP_ROWS = 4096                        # --dump-outputs: rows per workload, so that the three workloads stay under 64 MB of float32
 KERNEL_SOURCES = ["lifelike_agility_and_play_b200/csrc/llq_step16.cuh", "lifelike_agility_and_play_b200/csrc/llq_kernels.cuh", "lifelike_agility_and_play_b200/csrc/llq_cuda.cu",
                   "lifelike_agility_and_play_b200/csrc/llq_math.cuh"]
 
@@ -70,7 +71,12 @@ def parse():
     ap.add_argument("--element", type=int, default=3, help="EPMC element_id (0 flat joystick arena, 1 hurdles, 2 bars, 3 cubes)")
     ap.add_argument("--env", default="pmc", choices=["pmc", "epmc", "sepmc"],
                     help="headline workload: pmc = BASELINE configs[1]; epmc = configs[2] (8192 envs); sepmc = configs[4] (4096 pairs; --envs counts robots)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="GPU arm: write what the last timed step returned (observation, action, reward, done of every workload) as "
+                         "DIR/<workload>_<name>.npy; with several ranks, rank 0's shard")
     a = ap.parse_args()
+    if a.dump_outputs and a.impl == "reference":
+        ap.error("--dump-outputs records the GPU arm's timed path; it is not available with --impl reference")
     ELEMENT[0] = a.element
     if a.envs == 0:
         a.envs = 4096 if a.env == "pmc" else 8192
@@ -107,7 +113,7 @@ def action_pool_np(n, count, seed):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -337,7 +343,7 @@ def measure(args, env, n, ctx, headline):
         row = (xch.slab() if xch is not None else one_slab)[t]
         # the fused kernel writes the whole record (observation, action, reward, done) straight into the trajectory slab row
         eng.step_device(pool[i % POOL].data_ptr(), row.data_ptr(), reward.data_ptr(), done.data_ptr(), obs_ld=traj_w, stream=stream)
-        state["i"] = i + 1
+        state["i"], state["row"] = i + 1, row
         if t == UNROLL - 1 and do_gather:
             xch.hand_over()                 # unroll complete: it travels on the side stream while the next one is stepped
 
@@ -368,6 +374,14 @@ def measure(args, env, n, ctx, headline):
     wall = time.perf_counter() - wall0
     step_ms = sum(a.elapsed_time(b) for a, b in zip(ev0, ev1))
     c1 = eng.counters()
+    dump = None
+    if args.dump_outputs:
+        # the last timed step's record, read before anything else steps the engine; batches above DUMP_ROWS are sampled
+        # with a fixed seed so that the files stay small and two runs with the same arguments hold the same rows
+        sel = np.arange(n) if n <= DUMP_ROWS else np.sort(np.random.default_rng(0).choice(n, DUMP_ROWS, replace=False))
+        rec = state["row"].cpu().numpy()[sel]
+        dump = {"obs": rec[:, :ow], "action": rec[:, ow:ow + 12], "reward": reward.cpu().numpy()[sel],
+                "done": done.cpu().numpy()[sel].astype(np.float32)}
 
     # hot (no flush, back-to-back) variant: what a resident rollout loop sees
     h0, h1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -463,7 +477,7 @@ def measure(args, env, n, ctx, headline):
         e2e_pageable = nu * 32 / (time.perf_counter() - t2)
     res = {"env": env, "n": n, "nu": nu, "ow": ow, "step_ms": step_ms, "hot_ms": hot_ms, "kern_ms": kern_ms, "reset_ms": reset_ms,
            "e2e_s": e2e_s, "e2e_dev_obs_s": e2e_dev_obs_s, "e2e_steps": e2e_steps, "e2e_pageable": e2e_pageable, "wall": wall,
-           "launches": int(c1[4] - c0[4]), "gather": gather, "clocks": sampler.summary() if sampler else None,
+           "launches": int(c1[4] - c0[4]), "gather": gather, "clocks": sampler.summary() if sampler else None, "dump": dump,
            "limit_rows_per_env_substep": float(c1[3] - c0[3]) / max(1, nu * ROBOTS_PER_ENV[env] * args.steps * 10),
            "contact_rows_per_env_substep": float(c1[2] - c0[2]) / max(1, nu * ROBOTS_PER_ENV[env] * args.steps * 10)}
     if headline:
@@ -610,7 +624,7 @@ def assemble(args, r, world, peak, peak_src, reduce_max):
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
                      "traffic_note": traffic_note, "kernel": kernel_name(env), "kernel_ms": kern_ms, "reset_kernel_ms": reset_ms,
                      "algorithmic_bytes_per_env_step": ALGO_BYTES[akey], "peak_source": peak_src,
-                     "note": "latency/issue bound by design (SURVEY 7): ~2e5 flop per 1.7 kB of state; see profiles/"},
+                     "note": "latency/issue bound by design (SURVEY 7): ~2e5 flop per 1.7 kB of state"},
         "workload_stats": {"limit_rows_per_robot_substep": r["limit_rows_per_env_substep"], "contact_rows_per_robot_substep": r["contact_rows_per_env_substep"]},
     }
     if r["e2e_pageable"] is not None:
@@ -642,7 +656,7 @@ def main():
     torch.cuda.set_stream(bench_stream)
     assert bench_stream.cuda_stream != 0
     ctx = {"dev": dev, "rank": rank, "world": world, "local_rank": local_rank, "stream": bench_stream,
-           "flush": torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)}          # > 126 MB L2
+           "flush": torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)}          # > 50 MB L2 of the H100
 
     def reduce_max(vals):
         t = torch.tensor(vals, device=dev, dtype=torch.float64)
@@ -664,8 +678,8 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+    peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 3350 GB/s (H100 SXM data sheet, HBM3)"
     h = assemble(args, head, world, peak, peak_src, reduce_max)
     sub_out = {k: assemble(args, v, world, peak, peak_src, reduce_max) for k, v in subs.items()}
     numa_all = [numa]
@@ -676,6 +690,11 @@ def main():
         if world > 1:
             dist.destroy_process_group()
         return
+    if args.dump_outputs:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for key, r in [(args.env, head)] + list(subs.items()):
+            for name, arr in r["dump"].items():
+                np.save(os.path.join(args.dump_outputs, "%s_%s.npy" % (key, name)), np.ascontiguousarray(arr, dtype=np.float32))
 
     env = args.env
     do_gather = world > 1 and not args.no_gather

@@ -12,7 +12,7 @@
  *
  * Two shared libraries implement this header with identical semantics:
  *   oracle/libllq_cpu.so                                  fp64 CPU restatement (test oracle only)
- *   lifelike_agility_and_play_b200/csrc/libllq_cuda.so    fp32 sm_100a CUDA engine (the product)
+ *   lifelike_agility_and_play_b200/csrc/libllq_cuda.so    fp32 sm_90a CUDA engine (the product)
  *
  * Conventions: plain C types only; all array arguments are caller-owned;
  * every function returns 0 on success and a negative LLQ_E* code on failure,

@@ -124,7 +124,7 @@ _cuda_lib = None
 
 
 def load_cuda_library() -> LlqLibrary:
-    """Load the sm_100a engine.  No fallback: a missing build is a hard error."""
+    """Load the sm_90a engine.  No fallback: a missing build is a hard error."""
     global _cuda_lib
     if _cuda_lib is None:
         if not os.path.exists(CUDA_LIB_PATH):

@@ -1,7 +1,7 @@
-// llq_cuda.cu -- host side of the sm_100a rollout engine and its C-ABI (include/llq.h).
+// llq_cuda.cu -- host side of the sm_90a rollout engine and its C-ABI (include/llq.h).
 //
 // Build (see __graft_entry__.build):
-//   nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 -prec-div=false -prec-sqrt=false -Xcompiler -fPIC -shared \
+//   nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -prec-div=false -prec-sqrt=false -Xcompiler -fPIC -shared \
 //        -o libllq_cuda.so llq_cuda.cu
 //
 // This file holds no physics: it owns device memory (structure-of-arrays state, mocap table, model constants),

@@ -1,4 +1,4 @@
-// llq_math.cuh -- small fixed-size linear algebra for the sm_100a rollout kernels (fp32, registers only).
+// llq_math.cuh -- small fixed-size linear algebra for the sm_90a rollout kernels (fp32, registers only).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -153,7 +153,7 @@ LLQ_DI Q4 rotvec_q(V3 r) {
 }
 
 // 6x6 symmetric positive definite: packed lower Cholesky factor L (row-major lower triangle, 21 entries).
-// LLQ_CHOL_T selects the arithmetic of the factorisation and of the triangular solves (float by default; B200 runs
+// LLQ_CHOL_T selects the arithmetic of the factorisation and of the triangular solves (float by default; the H100 runs
 // fp64 FMA at half the fp32 rate, so -DLLQ_CHOL_T=double is affordable for these ~250 flops per sub-step).
 #ifndef LLQ_CHOL_T
 #define LLQ_CHOL_T float

@@ -1,4 +1,4 @@
-// llq_policy.cu -- on-device forward of the PMC actor (include/llq_policy.h; SURVEY.md 8 row f2), sm_100a.
+// llq_policy.cu -- on-device forward of the PMC actor (include/llq_policy.h; SURVEY.md 8 row f2), sm_90a.
 //
 // One CTA (256 threads = 8 warps) owns a tile of M = 32 observation rows and walks the whole net with the activations in
 // shared memory ([row][feature], padded so that the MMA A-fragment loads are conflict free).  The fully connected layers run
@@ -7,11 +7,11 @@
 // accuracy (the 12 outputs are joint targets for the physics and the parity bar is 1e-4, so plain TF32 -- a 1e-3 perturbation that
 // can also flip the discrete code -- is not an option).  The weights are re-ordered once, at llq_policy_create, into MMA
 // B-fragment order, so a warp fetches the fragments of a k-step with one coalesced 8-byte load per lane and n-tile; they stream
-// through L2 (1.4 MB per CTA) double-buffered in registers four k-steps ahead (A/B on the B200: eight or two k-steps per buffer and
-// `prefetch.global.L1` of the following group / of the next layer's head were all 3-10 % slower; profiles/r01_policy_ab.txt).  The previous version of this kernel did the same
-// layers with fp32 FFMA (one output neuron per thread, 32 accumulators): 0.137 ms per 4096 rows.
-// The tile is 32 rows, not 128, on purpose: 4096 envs -> 128 CTAs = one wave over the 148 SMs; a tcgen05 tile (M = 128) would
-// leave 116 SMs idle at this batch.  The 32-code search, the 256 -> 1 value output and the Gaussian sampling stay on the CUDA cores.
+// through L2 (1.4 MB per CTA) double-buffered in registers four k-steps ahead (LLQ_POLICY_KU).  An earlier version of this kernel
+// did the same layers with fp32 FFMA (one output neuron per thread, 32 accumulators).
+// The tile is 32 rows, not 128, on purpose: 4096 envs -> 128 CTAs = one wave over the H100's 132 SMs; a 128-row tile (one
+// wgmma M = 64 pair per warpgroup) would leave 100 SMs idle at this batch.  The 32-code search, the 256 -> 1 value output and the
+// Gaussian sampling stay on the CUDA cores.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string.h>
@@ -43,8 +43,8 @@ struct Weights {
 
 // x = hi + lo with hi = x truncated to TF32 (one LOP3) and lo = x - hi (exact in fp32, <= 13 significant bits).  The tensor
 // core reads only the TF32 bits of an operand register, i.e. it truncates lo to 11 significant bits itself: the dropped part
-// is <= 2^-21 |x|, the same order as the a_lo * b_lo product 3xTF32 leaves out.  (cvt.rna.tf32.f32 is emulated with ~5
-// integer instructions per value on sm_100a: with it the splits, not the MMAs, filled the issue slots.)
+// is <= 2^-21 |x|, the same order as the a_lo * b_lo product 3xTF32 leaves out.  (Truncation costs one LOP3
+// per value where a rounding cvt.rna.tf32.f32 split costs several instructions: the splits must not fill the issue slots.)
 __device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
   hi = __float_as_uint(x) & 0xffffe000u;
   lo = __float_as_uint(x - __uint_as_float(hi));

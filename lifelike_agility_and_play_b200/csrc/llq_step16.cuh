@@ -24,8 +24,9 @@
 namespace llq {
 
 #ifndef LLQ16_BLOCK
-#define LLQ16_BLOCK 224   // 14 envs per CTA: 4096 envs = 293 CTAs = one wave of 2 CTAs (14 warps) per SM; 256 would put 16 warps on 108 of the
-                          // 148 SMs (0.263 -> 0.247 ms); 128 / 160 threads: 0.256 / 0.249 ms (DESIGN.md 4.1)
+#define LLQ16_BLOCK 256   // 16 envs per CTA, 2 CTAs per SM: 4096 envs = 256 CTAs = one wave on the H100's 132 SMs (264 slots); 224
+                          // threads (293 CTAs) need a second wave there, 128 threads are one wave too but slower on EPMC / SEPMC
+                          // (DESIGN.md 4.1).  The size fixes which envs are paired in a warp, hence the order of an env's lane sums.
 #endif
 #ifndef LLQ16_MINB
 #define LLQ16_MINB 4   // resident CTAs per SM the register budget is sized for (4 x 128 threads x 128 registers = the whole file)

@@ -22,7 +22,7 @@ _FULL_PROP_SIZE = {'joint_pos': 12, 'joint_vel': 12, 'root_lin_vel_loc': 3, 'roo
 
 
 def _default_engine_factory(n_envs, model_blob, mocap, **cfg):
-    """Product path: the sm_100a engine, or a hard error (no CPU fallback)."""
+    """Product path: the sm_90a engine, or a hard error (no CPU fallback)."""
     return capi.VecEngine(capi.load_cuda_library(), n_envs, model_blob, mocap, **cfg)
 
 

@@ -1,4 +1,4 @@
-"""T2/T3: CUDA engine vs CPU oracle through the C-ABI (the parity tests proper; run with -m gpu on the B200 box).
+"""T2/T3: CUDA engine vs CPU oracle through the C-ABI (the parity tests proper; run with -m gpu on an H100).
 
 Tolerance (BASELINE.json north_star): 1e-4 relative.  "Relative" is taken per observation block (prop / future) and per
 state block against the block's max-norm, floor 1 -- the reference's own observation consumer normalises per block.
