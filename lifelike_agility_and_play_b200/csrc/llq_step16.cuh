@@ -38,7 +38,8 @@ struct alignas(16) SphTable { int n; int rule; int pad[2]; SphConst s[kMaxSph]; 
 // per-env shared-memory tables (floats)
 constexpr int kLinkTab = 12 * 8;      // link (3 k + i): c1 s1 cy sy | p(3) | -
 constexpr int kLegTab = 4 * 48;       // leg k: dynamics phase F(18) Hrow(9) rhs(3) Ic(10) facc(6); rows phase W(18) L(3) dinv(3) qd(3)
-constexpr int kConW = 20, kConTab = kMaxCon * kConW;   // contact: leg depth | Pc(3) n(3) t1(3) t2(3) | dist mu lam0 lam
+constexpr int kConW = 20, kConTab = kMaxCon * kConW;   // contact: leg depth | Pc(3) n(3) t1(3) t2(3) | dist mu lam0 lam | - -
+                                                       // (during the friction pass: ... lam0 | mu lam_n | lam_t1 lam_t2)
 constexpr int kLimTab = kMaxLim * 4;  // limit row: leg joint dir pen
 constexpr int kRowW = 12, kRowTab = 32 * kRowW;        // row: y(6) e(3) leg - -   (aliased by the 16 x 20 float scratch of the dynamics phase)
 constexpr int kEnvTab = 56;           // p_base(6) - - | Cholesky factor of the base block (21) - - - | joint targets (12) | actions (12)
@@ -264,8 +265,21 @@ LLQ_DI float delassus_entry(const RowRegs& r, const float* rw) {
   const float jt = r.wj[0] * bq.z + r.wj[1] * bq.w + r.wj[2] * cq4.x;
   return dot6(r.y, ys) + (__float_as_int(cq4.y) == r.leg ? jt : 0.f);
 }
+// One round of the recursive-halving reduction: the N partial sums a lane holds are split between it and its partner (lane ^ x),
+// which holds the same N sums of the neighbouring lanes.  The lower lane keeps u[0 .. M), the upper one u[N - M .. N); when N is odd
+// the middle value is kept (and summed) by both.  Every kept value is own + partner's, exactly as in a butterfly.
+template <int N>
+LLQ_DI void halve_sums(const float (&u)[N], float (&o)[(N + 1) / 2], bool upper, int x) {
+  constexpr int M = (N + 1) / 2;
+#pragma unroll
+  for (int j = 0; j < M; j++) {
+    const float lo = u[j], hi = j + M < N ? u[j + M] : u[j];
+    o[j] = (upper ? hi : lo) + __shfl_xor_sync(FULL, upper ? lo : hi, x);
+  }
+}
 // total impulse of an env: Yt += sum lam_r y_r and, per leg, sum lam_r w_r -- 18 values.  Rows that sit on the partner's half-warp are
-// handed across first (xor 16), then a butterfly over each half-warp.
+// handed across first (xor 16), then each half-warp reduces by recursive halving in the order of a butterfly (xor 1, 2, 4, 8): every
+// total is the same tree of additions, but a lane exchanges 9 + 5 + 3 + 2 values instead of 4 x 18, and ends with two of the totals.
 LLQ_DI void impulse_sums(const RowsIn& in, const RowRegs& r) {
   float v18[18];
 #pragma unroll
@@ -284,15 +298,18 @@ LLQ_DI void impulse_sums(const RowsIn& in, const RowRegs& r) {
       v18[t] = mine + __shfl_xor_sync(FULL, give, 16);
     }
   }
-#pragma unroll 1
-  for (int o = 1; o < 16; o <<= 1) {
-#pragma unroll
-    for (int t = 0; t < 18; t++) v18[t] += __shfl_xor_sync(FULL, v18[t], o);
-  }
-  if (in.res && (in.lane & 15) == 0) {                    // the lower half-warp holds env A's totals, the upper one env B's
-    st4(in.res, v18[0], v18[1], v18[2], v18[3]); st4(in.res + 4, v18[4], v18[5], v18[6], v18[7]);
-    st4(in.res + 8, v18[8], v18[9], v18[10], v18[11]); st4(in.res + 12, v18[12], v18[13], v18[14], v18[15]);
-    in.res[16] = v18[16]; in.res[17] = v18[17];
+  const bool b0 = in.lane & 1, b1 = in.lane & 2, b2 = in.lane & 4, b3 = in.lane & 8;
+  float v9[9], v5[5], v3[3], v2[2];
+  halve_sums<18>(v18, v9, b0, 1);
+  halve_sums<9>(v9, v5, b1, 2);
+  halve_sums<5>(v5, v3, b2, 4);
+  halve_sums<3>(v3, v2, b3, 8);
+  // Which totals a lane ends with, traced back through the rounds: v2[0] is v3[2 b3], v2[1] the shared v3[1]; v3[j] is v5[j + 3 b2]
+  // (j < 2) or the shared v5[2]; v5[j] is v9[j + 5 b1] (j < 4) or the shared v9[4]; v9[j] is v18[j + 9 b0].  A value kept by both
+  // lanes of a round is reported by the lower one, so each of the 18 totals is written once.
+  if (in.res) {                                           // the lower half-warp holds env A's totals, the upper one env B's
+    if (!(b3 && b2)) in.res[9 * b0 + 5 * b1 + (b3 ? 2 : 3 * b2)] = v2[0];
+    if (!b3 && !(b2 && b1)) in.res[9 * b0 + (b2 ? 4 : 1 + 5 * b1)] = v2[1];
   }
 }
 
@@ -313,15 +330,17 @@ LLQ_DI void solve_rows(const RowsIn& in) {
     const float* rowtab = in.tb + kLinkTab + kLegTab + kConTab + kLimTab;
     const int ncon = 3 * nc;
 #pragma unroll 1
-    for (int col = 0; col < 3 * Ce; col++) {
-      const float a = delassus_entry(r, rowtab + col * kRowW);
-      acol[col * 32] = col < ncon ? a : 0.f;        // (beyond the env's list the table holds old rows: finite, masked)
+    for (int col = 0; col < 3 * Ce; col += 2) {     // two columns per iteration (3 Ce and Le are even)
+      const float a0 = delassus_entry(r, rowtab + col * kRowW), a1 = delassus_entry(r, rowtab + (col + 1) * kRowW);
+      acol[col * 32] = col < ncon ? a0 : 0.f;       // (beyond the env's list the table holds old rows: finite, masked)
+      acol[(col + 1) * 32] = col + 1 < ncon ? a1 : 0.f;
     }
     const float* rl = rowtab + ncon * kRowW;
 #pragma unroll 1
-    for (int t = 0; t < Le; t++) {
-      const float a = delassus_entry(r, rl + t * kRowW);
-      acol[(24 + t) * 32] = t < nl ? a : 0.f;
+    for (int t = 0; t < Le; t += 2) {
+      const float a0 = delassus_entry(r, rl + t * kRowW), a1 = delassus_entry(r, rl + (t + 1) * kRowW);
+      acol[(24 + t) * 32] = t < nl ? a0 : 0.f;
+      acol[(25 + t) * 32] = t + 1 < nl ? a1 : 0.f;
     }
   }
   // warm start of the normal rows
@@ -331,57 +350,70 @@ LLQ_DI void solve_rows(const RowsIn& in) {
   // projected Gauss-Seidel (btMultiBodyConstraintSolver::solveSingleIteration order).  One row update: candidate on every lane (only
   // the owner's counts), owner commits, broadcast, one LDS + FMA per lane.  Dependent chain per row: FFMA (candidate from
   // c = lam + rhs, kept up to date off the chain) -> 2 FMNMX -> FADD -> SHFL -> FFMA.
+  // Step t of a loop broadcasts from source lane s (the env's first row of that kind + t; the loops are padded to the warp-uniform
+  // bound); a lane commits where s equals its own position in that loop (-1: no row there), one compare per row.  A padded step broadcasts some lane's finite increment, which meets
+  // a zero coefficient column and leaves b as it is.
+  const bool is_con = in.rr < 3 * nc, is_lim = !is_con && in.rr < 3 * nc + nl;
+  const int d = in.rr % 3;
+  const int at_lim = is_lim ? lane : -1, at_nrm = is_normal ? lane : -1;
+  const int at_fric = is_con && d != 0 ? lane - d : -1;      // a tangent row commits at its contact's step, whose source lane is the normal's
+  float* const cfric = in.tb + kLinkTab + kLegTab + 16;       // per contact: lam0 | cone radius mu lam_n | impulses of the two tangents
   float rc = r.lam + r.rhs;
 #define LLQ16_CLAMP_LIMIT(x) fminf(fmaxf((x), 0.f), r.hi)      /* joint-limit rows: [0, max impulse] */
 #define LLQ16_CLAMP_NORMAL(x) fmaxf((x), 0.f)                  /* normal rows: [0, 1e10] -- the upper bound never binds a finite state */
-#define LLQ16_ROW_UPDATE(src, a, valid, CLAMP)                                                        \
+#define LLQ16_ROW_UPDATE(s, a, at, CLAMP)                                                             \
   {                                                                                                   \
     const float cl = CLAMP(fmaf(-r.b, r.invd, rc));      /* clamp the accumulated impulse */           \
     const float dl = cl - r.lam;                                                                      \
-    const bool own = lane == (src) && (valid);                                                        \
+    const bool own = (s) == (at);                                                                     \
     r.lam = own ? cl : r.lam;                                                                         \
     rc = own ? cl + r.rhs : rc;                                                                       \
-    r.b = fmaf((a), __shfl_sync(FULL, dl, (src)), r.b);                                               \
+    r.b = fmaf((a), __shfl_sync(FULL, dl, (s)), r.b);                                                 \
   }
 #pragma unroll 1
   for (int it = 0; it < in.iters; it++) {
+    // (the loops count with a warp-uniform t: with a per-lane bound the compiler could not prove the shuffles convergent)
     {
-      int src = lane0 + 3 * nc;
-      const float* ap = acol + 24 * 32;
+      const int s0 = lane0 + 3 * nc;
 #pragma unroll 1
-      for (int t = 0; t < Le; t += 2, src += 2, ap += 64) {     // joint-limit rows in joint order
-        LLQ16_ROW_UPDATE(src, ap[0], t < nl, LLQ16_CLAMP_LIMIT)
-        LLQ16_ROW_UPDATE(src + 1, ap[32], t + 1 < nl, LLQ16_CLAMP_LIMIT)
+      for (int t = 0; t < Le; t += 2) {                         // joint-limit rows in joint order
+        const float* ap = acol + (24 + t) * 32;
+        LLQ16_ROW_UPDATE(s0 + t, ap[0], at_lim, LLQ16_CLAMP_LIMIT)
+        LLQ16_ROW_UPDATE(s0 + t + 1, ap[32], at_lim, LLQ16_CLAMP_LIMIT)
       }
     }
     {
-      int src = lane0;
-      const float* ap = acol;
 #pragma unroll 1
-      for (int t = 0; t < Ce; t += 2, src += 6, ap += 192) {    // normal rows in contact order
-        LLQ16_ROW_UPDATE(src, ap[0], t < nc, LLQ16_CLAMP_NORMAL)
-        LLQ16_ROW_UPDATE(src + 3, ap[96], t + 1 < nc, LLQ16_CLAMP_NORMAL)
+      for (int t = 0; t < Ce; t += 2) {                         // normal rows in contact order
+        const float* ap = acol + 96 * t;
+        LLQ16_ROW_UPDATE(lane0 + 3 * t, ap[0], at_nrm, LLQ16_CLAMP_NORMAL)
+        LLQ16_ROW_UPDATE(lane0 + 3 * t + 3, ap[96], at_nrm, LLQ16_CLAMP_NORMAL)
       }
     }
     {
-      int src = lane0;
-      const float* ap = acol;
+      // The cone radius and the tangent impulses of every contact are fixed during this pass until its own step: they go through the
+      // contact records (one float4 per step, off the dependent chain) instead of three shuffles per step.  Records beyond the env's
+      // contacts hold finite values of earlier sub-steps (zeros at the start of the kernel).
+      __syncwarp();                                           // the previous pass's reads of the records are done
+      if (is_con) cfric[(in.rr / 3) * kConW + 1 + d] = d == 0 ? r.mu * r.lam : r.lam;
+      __syncwarp();
 #pragma unroll 1
-      for (int t = 0; t < in.Cmax; t++, src += 3, ap += 96) {   // friction pairs with the implicit cone (resolveConeFrictionConstraintRows)
-        // One shuffle round trip on the dependent chain: the two tangent rows' candidates go to every lane together with their current
-        // impulses and the cone's radius (those three do not depend on this step's b), and every lane forms both increments itself.
+      for (int t = 0; t < in.Cmax; t++) {                       // friction pairs with the implicit cone (resolveConeFrictionConstraintRows)
+        // One shuffle round trip on the dependent chain: the two tangent rows' candidates go to every lane, and every lane forms both
+        // increments itself.
+        const int s = lane0 + 3 * t;
+        const float* ap = acol + 96 * t;
         const float sown = fmaf(-r.b, r.invd, rc);
-        const float sa = __shfl_sync(FULL, sown, src + 1), sb = __shfl_sync(FULL, sown, src + 2);
-        const float la = __shfl_sync(FULL, r.lam, src + 1), lb = __shfl_sync(FULL, r.lam, src + 2);
-        const float limit = __shfl_sync(FULL, r.mu * r.lam, src);
+        const float sa = __shfl_sync(FULL, sown, s + 1), sb = __shfl_sync(FULL, sown, s + 2);
+        const float4 cq = ld4(cfric + t * kConW);
+        const float limit = cq.y, la = cq.z, lb = cq.w;
         const float r2 = sa * sa + sb * sb;
         const float rs = rsqrtf(r2);                           // issued before the comparison resolves (inf for r2 = 0: not selected)
         const bool clip = r2 >= limit * limit && r2 > 0.f;
         const float sc = limit * rs;
         const float na = clip ? sa * sc : sa, nb = clip ? sb * sc : sb;
-        const bool valid = t < nc;
-        if (lane == src + 1 && valid) { r.lam = na; rc = na + r.rhs; }
-        if (lane == src + 2 && valid) { r.lam = nb; rc = nb + r.rhs; }
+        const float nown = d == 1 ? na : nb;
+        if (s == at_fric) { r.lam = nown; rc = nown + r.rhs; }
         r.b = fmaf(ap[32], na - la, fmaf(ap[64], nb - lb, r.b));
       }
     }
@@ -394,6 +426,7 @@ LLQ_DI void solve_rows(const RowsIn& in) {
   if (is_normal) in.tb[kLinkTab + kLegTab + (in.rr / 3) * kConW + 17] = r.lam;
   __syncwarp();                     // every lane is done with the row table: its head becomes the result area
   impulse_sums(in, r);
+  T16_IN(3);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -696,7 +729,7 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
   __shared__ __align__(16) SphTable ST;
   __shared__ __align__(16) float s_new[EPT][kNewObs];
   __shared__ __align__(16) float s_hist[EPT][kHist];
-  __shared__ int s_cnt[32];                                   // contacts | limit rows << 8 of the CTA's envs, this sub-step
+  __shared__ __align__(16) int s_cnt[32];                     // contacts | limit rows << 8 | sort key << 16 of the CTA's envs, this sub-step
   extern __shared__ __align__(16) float s_env_dyn[];   // [EPB][kEnvFloats] per-env tables, then one kATabWarp coefficient table per warp
   const int tid = threadIdx.x;
   const int N = P.n_envs;
@@ -728,6 +761,7 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
   float* const envtab = rowtab + kRowTab;
   float* const s_atab = s_env_dyn + EPB * kEnvFloats;   // [BLOCK / 32][32 cols][32 lanes] Delassus coefficients, one table per warp
   for (int col = 0; col < 32; col++) s_atab[(tid >> 5) * kATabWarp + col * 32 + (tid & 31)] = 0.f;      // finite from the start (masked steps multiply them by 0)
+  for (int t = l16; t < kConTab; t += 16) contab[t] = 0.f;      // so are the contact records the friction sweep reads on its padded steps
   // joints with a lower dof index than this lane's (k, i): rank of a violated limit in Bullet's row order
   unsigned lowmask = 0;
 #pragma unroll
@@ -1280,7 +1314,8 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
     T16_MARK(2);
     float dvb[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, dvl[3] = {0.f, 0.f, 0.f};
     // ---------------- the rows of the CTA's envs: publish the counts, pair the envs by load, solve, hand the totals back
-    if (l16 == 0) s_cnt[el] = nc | (nl << 8);
+    // contacts | limit rows << 8 | a sort key above them: row count, ties to the lower env index (all keys differ)
+    if (l16 == 0) s_cnt[el] = nc | (nl << 8) | ((32 * (3 * nc + nl) + 31 - el) << 16);
     __syncthreads();           // every env's tables (links, legs, contacts, limits, Cholesky factor, predicted velocity) are complete
     T16_MARK(0);
     {
@@ -1290,19 +1325,18 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
       // its own tables).
       const int lane = tid & 31, wq = tid >> 5;
       const int cnt = lane < EPB ? s_cnt[lane] : 0;
-      const int nrow = 3 * (cnt & 255) + (cnt >> 8);
       int rank = 0;
-#pragma unroll 1
-      for (int j = 0; j < EPB; j++) {
-        const int nj = __shfl_sync(FULL, nrow, j);
-        rank += (nj > nrow || (nj == nrow && j < lane)) ? 1 : 0;
+#pragma unroll
+      for (int j = 0; j < EPB; j += 4) {
+        const int4 c4 = *reinterpret_cast<const int4*>(s_cnt + j);
+        rank += (c4.x > cnt) + (j + 1 < EPB && c4.y > cnt) + (j + 2 < EPB && c4.z > cnt) + (j + 3 < EPB && c4.w > cnt);
       }
       const int ea = __ffs(__ballot_sync(FULL, lane < EPB && rank == wq)) - 1;
       const int eb = __ffs(__ballot_sync(FULL, lane < EPB && rank == EPB - 1 - wq)) - 1;
       const int ca_ = __shfl_sync(FULL, cnt, ea), cb_ = __shfl_sync(FULL, cnt, eb);
       // (redux results live in uniform registers: the guards below compile to uniform branches)
-      const int cA = __reduce_max_sync(FULL, ca_ & 255), lA = __reduce_max_sync(FULL, ca_ >> 8);
-      const int cB = __reduce_max_sync(FULL, cb_ & 255), lB = __reduce_max_sync(FULL, cb_ >> 8);
+      const int cA = __reduce_max_sync(FULL, ca_ & 255), lA = __reduce_max_sync(FULL, (ca_ >> 8) & 255);
+      const int cB = __reduce_max_sync(FULL, cb_ & 255), lB = __reduce_max_sync(FULL, (cb_ >> 8) & 255);
       const int eA = __reduce_max_sync(FULL, ea), eB = __reduce_max_sync(FULL, eb);
       const int nA = 3 * cA + lA, nB = 3 * cB + lB;
       T16_ADD(6, max(cA, cB) * 256 + max(lA, lB) + (nA > 16 || nB > 16 ? 65536 : 0) + (nA + nB > 32 ? (1 << 24) : 0));
@@ -1332,8 +1366,9 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
         }
       }
     }
-    __syncthreads();           // the totals of every env of the CTA are in its row table
     T16_MARK(3);
+    __syncthreads();           // the totals of every env of the CTA are in its row table
+    T16_MARK(11);
     if (nc | nl) {
       if (l16 == 0) { n_contact_rows += 3u * (unsigned)nc; n_limit_rows += (unsigned)nl; }
 #pragma unroll
