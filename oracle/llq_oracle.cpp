@@ -610,6 +610,7 @@ bool physics_substep(llq_engine& E, Env& e, const double* tau, int64_t* n_contac
       double pen = side == 0 ? e.q[j] - l.lower : l.upper - e.q[j];
       e.margin = std::min(e.margin, std::fabs(pen));
       if (pen > 0) continue;                       // btMultiBodyJointLimitConstraint: row only when violated
+      e.margin = std::min(e.margin, std::fabs(pen + 0.04));   // the split-impulse threshold below switches the positional term
       double dir = side == 0 ? 1.0 : -1.0;
       Row r; std::memset(&r, 0, sizeof(r));
       r.J[6 + j] = dir;

@@ -81,12 +81,18 @@ def test_a_folded_robot_rests_on_its_trunk(oracle_lib, blob, small_mocap):
 def test_heavy_ctas_match_the_oracle(built, blob, small_mocap, oracle_lib):
     """Every robot of the batch lies folded on the ground with joints pushed against (and beyond) their stops: 20-32 constraint rows per
     robot, so that rows spill over into the partner's lanes and pairs exceed the warp's 32 lanes (the two-pass path of the solver, which
-    the benchmark's regime never reaches once the robots are paired by load).  Teacher-forced against the oracle like the other parity tests."""
+    the benchmark's regime never reaches once the robots are paired by load).  Teacher-forced against the oracle like the other parity tests.
+    The per-element comparison of these paths, without near-branch exclusions, is tests/test_solver_cases_gpu.py."""
+    import solver_cases as sc
     from test_parity_gpu import blockrel
-    n = 56                                            # 4 CTAs of 14 robots, every one of them heavy
+    n = 56                                            # 3 CTAs of 16 robots and a partly filled fourth (8 robots + 8 copies of the last)
     gpu = capi.VecEngine(capi.load_cuda_library(), n, blob, small_mocap, seed=5, auto_reset=0)
     cpu = capi.VecEngine(oracle_lib, n, blob, small_mocap, seed=5, auto_reset=0)
     cpu.reset(); gpu.reset()
+    # the first sub-step alone: its decisions are taken on the pose handed in, so the rows dropped by the caps must agree exactly
+    gpu1 = capi.VecEngine(capi.load_cuda_library(), n, blob, small_mocap, seed=5, auto_reset=0, substeps=1)
+    cpu1 = capi.VecEngine(oracle_lib, n, blob, small_mocap, seed=5, auto_reset=0, substeps=1)
+    cpu1.reset(); gpu1.reset()
     rng = np.random.default_rng(4)
 
     def heavy_state():
@@ -98,24 +104,35 @@ def test_heavy_ctas_match_the_oracle(built, blob, small_mocap, oracle_lib):
         q[:, 2::3] = 2.6 + 0.05 * rng.standard_normal((n, 4)).astype(np.float32)                                                 # knees beyond theirs
         st[:, 13:25] = q; st[:, 25:37] = 0.3 * rng.standard_normal((n, 12)).astype(np.float32)
         return st
-    c0 = gpu.counters().copy()
+    c0, k0 = gpu.counters().copy(), cpu.counters().copy()
     worst, ok_n, tot = 0.0, 0, 0
     for t in range(8):
-        cpu.set(capi.F_STATE, heavy_state()); cpu.set(capi.F_WARMSTART, np.zeros((n, 32), np.float32))      # a fresh heap every step
-        for f in (capi.F_STATE, capi.F_WARMSTART, capi.F_OBS, capi.F_TIME, capi.F_CLIP):
-            gpu.set(f, cpu.get(f))
+        st = heavy_state()
+        d = [sc.decisions(s, sc.Statics()) for s in st]
+        mapping, reached = sc.warp_cases([x["nc"] for x in d], [x["nl"] for x in d])
+        assert "two_pass" in reached, "the first sub-step of the heap must solve some pairs in two passes: %s" % sorted(reached)
         a = (0.3 * rng.standard_normal((n, 12))).astype(np.float32)
-        gpu.step(a); cpu.step(a)
+        dropped = sum(max(x["nc"] - sc.MAX_CON, 0) + max(x["nl"] - sc.MAX_LIM, 0) for x in d)
+        for g_, c_ in ((gpu1, cpu1), (gpu, cpu)):
+            c_.set(capi.F_STATE, st); c_.set(capi.F_WARMSTART, np.zeros((n, 32), np.float32))      # a fresh heap every step
+            for f in (capi.F_STATE, capi.F_WARMSTART, capi.F_OBS, capi.F_TIME, capi.F_CLIP):
+                g_.set(f, c_.get(f))
+            g0, k0_ = g_.counters()[5], c_.counters()[5]
+            g_.step(a); c_.step(a)
+            if g_ is gpu1:
+                assert g_.counters()[5] - g0 == c_.counters()[5] - k0_ == dropped, "rows beyond the caps are counted, not solved"
         e = blockrel(gpu.get(capi.F_STATE), cpu.get(capi.F_STATE))
         m = cpu.get(capi.F_DECISION_MARGIN)
         good = (e < 1e-4) | (m < 5e-4)
         ok_n += int(good.sum()); tot += n; worst = max(worst, float(np.percentile(e, 90)))
         wg, wc = gpu.get(capi.F_WARMSTART) > 0, cpu.get(capi.F_WARMSTART) > 0
         assert (wg != wc).mean() < 0.02
-    c1 = gpu.counters()
+    c1, k1 = gpu.counters(), cpu.counters()
     per_sub = ((c1[2] - c0[2]) + (c1[3] - c0[3])) / float(n * 8 * 10)
     assert per_sub > 17.0, "the scenario must be heavy: %.1f rows per robot and sub-step" % per_sub
-    assert (c1[5] - c0[5]) < 1.0 * n * 80                                # (rows beyond the caps are counted, not solved: same rule on both sides)
+    # over 10 sub-steps a contact within fp32 rounding of its branch may flip: the same 2 % as the warm-start sets above
+    assert abs((c1[5] - c0[5]) - (k1[5] - k0[5])) <= 0.02 * (k1[5] - k0[5]) + 2, (c1[5] - c0[5], k1[5] - k0[5])
     assert ok_n >= 0.98 * tot, (ok_n, tot, worst)
     print("heavy CTAs: %.1f rows per robot and sub-step, %d of %d env-steps within 1e-4 or next to a branch" % (per_sub, ok_n, tot))
-    gpu.close(); cpu.close()
+    for e_ in (gpu, cpu, gpu1, cpu1):
+        e_.close()
