@@ -4,6 +4,7 @@ import os
 import numpy as np
 import pytest
 
+import perception_cases as pc
 from lifelike_agility_and_play_b200 import _capi as capi
 from test_golden_epmc import EPMC_CFG, GOLD
 from test_parity_gpu import MU_A, SIGMA_A, TOL, blockrel
@@ -34,7 +35,20 @@ def test_epmc_reset_parity(built, blob, oracle_lib):
     gpu.close(); cpu.close()
 
 
-def _sweep(gpu, cpu, n, steps, rng):
+def _front_flips(og, oc, st, err_other):
+    """Env-steps whose only deviation is a percep_front ray that is not decisive under the fp64 caster on the oracle's post-step
+    pose (within 1e-4 m of the ground-plane branch): every other block within TOL, and every deviating front ray non-decisive."""
+    fg, fc = og[:, 588:913].astype(np.float64), oc[:, 588:913].astype(np.float64)
+    dev = np.abs(fg - fc) > TOL * np.maximum(1.0, np.abs(fc).max(1, keepdims=True))     # blockrel's normalisation, per value
+    out = np.zeros(len(og), bool)
+    for i in np.flatnonzero(dev.any(1) & (err_other < TOL)):
+        s = st[i].astype(np.float64)
+        dec = pc.rays_decisive(s[0:3], pc.rot(s[3:7]), pc.SLAB)[pc.N_DOWN + pc.N_1D:]
+        out[i] = not dec[dev[i]].any()
+    return out
+
+
+def _sweep(gpu, cpu, n, steps, rng, front=None):
     E, M, DD, MU = [], [], [], []
     for t in range(steps):
         a = np.clip(MU_A + SIGMA_A * rng.standard_normal((n, 12)).astype(np.float32), -1, 1).astype(np.float32)
@@ -47,6 +61,10 @@ def _sweep(gpu, cpu, n, steps, rng):
         e = np.maximum.reduce([blockrel(og[:, :135], oc[:, :135]), blockrel(og[:, 135:], oc[:, 135:]),
                                blockrel(gpu.get(capi.F_STATE), cpu.get(capi.F_STATE)),
                                np.abs(rg - rc) / np.maximum(1e-4, np.abs(rc)) * 1e-1])
+        if front is not None:
+            other = np.maximum.reduce([blockrel(og[:, :135], oc[:, :135]), blockrel(og[:, 135:588], oc[:, 135:588]), blockrel(og[:, 913:], oc[:, 913:]),
+                                       blockrel(gpu.get(capi.F_STATE), cpu.get(capi.F_STATE)), np.abs(rg - rc) / np.maximum(1e-4, np.abs(rc)) * 1e-1])
+            front.append(_front_flips(og, oc, cpu.get(capi.F_STATE), other))
         E.append(e); M.append(cpu.get(capi.F_DECISION_MARGIN)); DD.append(dg != dc); MU.append(ac[:, 13].copy())
         m = dc.astype(np.uint8)
         if m.any():
@@ -77,8 +95,11 @@ def test_epmc_substep_parity(built, blob, oracle_lib):
     # (measured: 1 / 3 / 10 / 30 iterations -> 21 / 53 / 65 / 139 deviating sub-steps of 143k, max 2.5e-4 / 6e-4 / 8e-3 / 0.45)
     gpu, cpu = _pair(n, blob, oracle_lib, 7, cmd_freq_lo=30, cmd_freq_hi=90, max_steps=400, substeps=1, solver_iters=1)
     gpu.reset(); cpu.reset()
-    e1, m1, dd1, mu1 = _sweep(gpu, cpu, n, steps, np.random.default_rng(3))
-    front_flip = e1 > 0.5          # a percep_front ray grazing the ground plane may hit on one side and miss on the other
+    front = []
+    e1, m1, dd1, mu1 = _sweep(gpu, cpu, n, steps, np.random.default_rng(3), front)
+    # a percep_front ray grazing the ground plane may hit on one side and miss on the other: such an env-step is excused only when
+    # nothing else deviates and every deviating front ray is within 1e-4 m of its branch (tests/perception_cases.py)
+    front_flip = np.concatenate(front)
     print("  with solver_iters = 1: %d above 1e-4, max %.1e" % (int(((e1 >= TOL) & ~front_flip).sum()), e1[~front_flip].max()))
     assert ((e1 >= TOL) & ~front_flip).mean() <= 3e-4 and e1[~front_flip].max() < 1e-3 and front_flip.sum() <= 3
     gpu.close(); cpu.close()
