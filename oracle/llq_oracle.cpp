@@ -936,7 +936,6 @@ double step_env(llq_engine& E, Env& e, const float* action, bool* done, int64_t*
              (cf.w_end_effector / sw) * std::exp(-40.0 * dee) +
              (cf.w_root_pose / sw) * std::exp(-20.0 * dp - 10.0 * angle * angle) +
              (cf.w_root_vel / sw) * std::exp(-2.0 * dvl - 0.2 * dva);
-  e.reward_sum += r;
   // termination PLE:337-348
   M3 R = qmat(q1);
   double left_z = R.m[0][2] * R.m[1][0] - R.m[1][2] * R.m[0][0];                             // LR:171-172
@@ -947,6 +946,7 @@ double step_env(llq_engine& E, Env& e, const float* action, bool* done, int64_t*
   bool diff = std::fabs(angle) > 1.0 || dp > 1.0;                                            // PLE:319-335
   *done = fall || ended || diff || ob_hit || !ok;                                            // PLE:347
   if (!ok || !std::isfinite(r)) { r = 0.0; *done = true; }
+  e.reward_sum += r;                  // after the zeroing: a NaN reward must not poison the sum and, through it, the clip table
   return r;
 }
 
