@@ -47,15 +47,35 @@ extern "C" {
                                  (max_game/chase_tag_game_env.py:111-124) */
 #define LLQ_ENV_SEPMC 2      /* ChaseTagGameEnv in the empty arena of the shipped config (max_game/chase_tag_game_env.py,
                                 train_scripts/example_sepmc_train.sh:113-116).  n_envs counts ROBOTS and must be even: robots 2p and
-                                2p+1 form env-pair p; actions / obs / reward / done are per robot (done is the pair's, on both rows).
-                                LLQ_F_AUX rows for SEPMC: counter, with_flag, flag_x, flag_y, control_spd, oppo_visible, switch_flag,
-                                total_spd, max_spd, push_count, push_fx..z (last applied), foot_friction, push_draws (pair), flag_draws,
-                                yaw_accum_deg (pair), flag_touch (this robot's body touched the flag in the last sub-step: the stale manifold
-                                reset() sees, CTG:302,573) */
-#define LLQ_AUX_DIM  18      /* LLQ_F_AUX: counter, cmd_vary_freq, target_x, target_y, target_spd, target_angle, last_pos_diff_len,
-                                total_spd, max_spd, push_count, push_fx, push_fy, push_fz, foot_friction, push_draws, cmd_draws,
-                                yaw_accum_deg (the reference mutates its module-level init-state dict, so reset yaws accumulate: PGE:181-189),
-                                init_pos_diff_len (elements 1-3, PGE:192-195) */
+                                2p+1 form env-pair p; actions / obs / reward / done are per robot (done is the pair's, on both rows). */
+#define LLQ_AUX_DIM  18      /* columns of LLQ_F_AUX, the EPMC / SEPMC bookkeeping; slots: */
+/* shared by EPMC and SEPMC */
+#define LLQ_AUX_COUNTER        0   /* env steps of the episode */
+#define LLQ_AUX_TOTAL_SPD      7   /* sum of the per-step speeds */
+#define LLQ_AUX_MAX_SPD        8   /* largest per-step speed */
+#define LLQ_AUX_PUSH_COUNT     9   /* push randomiser sub-step counter (PR:56-87) */
+#define LLQ_AUX_PUSH_F        10   /* last applied push force x; y and z in slots 11 and 12 */
+#define LLQ_AUX_FOOT_FRICTION 13   /* per-episode foot lateral friction (PGE:209) */
+#define LLQ_AUX_PUSH_DRAWS    14   /* push-randomiser draws taken (SEPMC: the pair's) */
+#define LLQ_AUX_YAW_ACCUM_DEG 16   /* running reset yaw: the reference mutates its module-level init-state dict (PGE:181-189; SEPMC: the pair's) */
+/* EPMC */
+#define LLQ_AUX_CMD_FREQ           1   /* cmd_vary_freq (PGE:170,223) */
+#define LLQ_AUX_TARGET_X           2
+#define LLQ_AUX_TARGET_Y           3
+#define LLQ_AUX_TARGET_SPD         4
+#define LLQ_AUX_TARGET_ANGLE       5
+#define LLQ_AUX_LAST_POS_DIFF_LEN  6
+#define LLQ_AUX_CMD_DRAWS         15   /* joystick-command draws taken */
+#define LLQ_AUX_INIT_POS_DIFF_LEN 17   /* elements 1-3 (PGE:192-195) */
+/* SEPMC */
+#define LLQ_AUX_WITH_FLAG     1
+#define LLQ_AUX_FLAG_X        2
+#define LLQ_AUX_FLAG_Y        3
+#define LLQ_AUX_CONTROL_SPD   4
+#define LLQ_AUX_OPPO_VISIBLE  5
+#define LLQ_AUX_SWITCH_FLAG   6
+#define LLQ_AUX_FLAG_DRAWS   15
+#define LLQ_AUX_FLAG_TOUCH   17   /* this robot's body touched the flag in the last sub-step: the stale manifold reset() sees (CTG:302,573) */
 #define LLQ_NUM_FEET    4
 
 /* error codes */

@@ -19,6 +19,12 @@ LLQ_IO_HOST, LLQ_IO_DEVICE, LLQ_IO_PINNED = 0, 1, 2
  F_AVG_REWARD, F_EPISODE_ID, F_FOOT_POS, F_DECISION_MARGIN, F_AUX, F_OB_ID, F_BOXES, F_NBOX) = range(17)
 MAX_BOXES = 36
 ENV_PMC, ENV_EPMC, ENV_SEPMC, OBS_DIM_EPMC, OBS_DIM_SEPMC, AUX_DIM = 0, 1, 2, 916, 965, 18
+# F_AUX columns (LLQ_AUX_* of include/llq.h): shared, then EPMC, then SEPMC meanings of slots 1-6, 15 and 17
+AUX_COUNTER, AUX_TOTAL_SPD, AUX_MAX_SPD, AUX_PUSH_COUNT, AUX_PUSH_F, AUX_FOOT_FRICTION, AUX_PUSH_DRAWS, AUX_YAW_ACCUM_DEG = 0, 7, 8, 9, 10, 13, 14, 16
+(AUX_CMD_FREQ, AUX_TARGET_X, AUX_TARGET_Y, AUX_TARGET_SPD, AUX_TARGET_ANGLE, AUX_LAST_POS_DIFF_LEN, AUX_CMD_DRAWS,
+ AUX_INIT_POS_DIFF_LEN) = 1, 2, 3, 4, 5, 6, 15, 17
+(AUX_WITH_FLAG, AUX_FLAG_X, AUX_FLAG_Y, AUX_CONTROL_SPD, AUX_OPPO_VISIBLE, AUX_SWITCH_FLAG, AUX_FLAG_DRAWS,
+ AUX_FLAG_TOUCH) = 1, 2, 3, 4, 5, 6, 15, 17
 
 # field id -> (dtype, per-env width or None for per-clip tables)
 _FIELDS = {

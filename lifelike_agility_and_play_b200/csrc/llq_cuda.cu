@@ -114,12 +114,13 @@ int ensure_scratch(llq_handle h, size_t bytes) {
 
 llq::MocapDev mocap_dev(llq_handle h) { return llq::MocapDev{h->d_frames, h->d_clip_off, h->n_clips, h->d_ob_table, h->d_ob_off}; }
 
-template <int BLOCK, int ENV>
+template <int ENV>
 void launch_reset_t(llq_handle h, const llq::EnvArrays& E, const llq::ResetParams& RP, float* obs2, long long ld, cudaStream_t s) {
+  constexpr int BLOCK = llq::kResetBlock;
   int threads = 4 * h->cfg.n_envs;
   int grid = (threads + BLOCK - 1) / BLOCK;
   size_t smem = sizeof(double) * (size_t)(h->n_clips > 0 ? h->n_clips : 1);
-  llq::pmc_reset_kernel<BLOCK, ENV><<<grid, BLOCK, smem, s>>>(E, mocap_dev(h), h->P, h->d_model, RP, obs2, ld);
+  llq::pmc_reset_kernel<ENV><<<grid, BLOCK, smem, s>>>(E, mocap_dev(h), h->P, h->d_model, RP, obs2, ld);
 }
 template <int ENV>
 int launch_step16(llq_handle h, const llq::EnvArrays& E, const float* a, float* obs2, long long ld, cudaStream_t s) {
@@ -143,10 +144,10 @@ int launch_step(llq_handle h, const llq::EnvArrays& E, const float* a, float* ob
   return epmc ? launch_step16<1>(h, E, a, obs2, ld, s) : launch_step16<0>(h, E, a, obs2, ld, s);
 }
 void launch_reset(llq_handle h, const llq::EnvArrays& E, const llq::ResetParams& RP, float* obs2, long long ld, cudaStream_t s) {
-  if (h->cfg.env_kind == LLQ_ENV_EPMC && h->cfg.element_id != 0) launch_reset_t<128, 3>(h, E, RP, obs2, ld, s);
-  else if (h->cfg.env_kind == LLQ_ENV_EPMC) launch_reset_t<128, 1>(h, E, RP, obs2, ld, s);
-  else if (h->cfg.env_kind == LLQ_ENV_SEPMC) launch_reset_t<128, 2>(h, E, RP, obs2, ld, s);
-  else launch_reset_t<128, 0>(h, E, RP, obs2, ld, s);
+  if (h->cfg.env_kind == LLQ_ENV_EPMC && h->cfg.element_id != 0) launch_reset_t<3>(h, E, RP, obs2, ld, s);
+  else if (h->cfg.env_kind == LLQ_ENV_EPMC) launch_reset_t<1>(h, E, RP, obs2, ld, s);
+  else if (h->cfg.env_kind == LLQ_ENV_SEPMC) launch_reset_t<2>(h, E, RP, obs2, ld, s);
+  else launch_reset_t<0>(h, E, RP, obs2, ld, s);
   h->counters[4]++;
 }
 

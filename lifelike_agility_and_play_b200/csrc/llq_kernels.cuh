@@ -10,6 +10,7 @@
 //   PlayGroundEnv reset / perception / rewards   max_game_elements/playground_env.py:196-249, 374-539; bullet_static_entities.py:170-500
 //   ChaseTagGameEnv reset / perception / game    max_game/chase_tag_game_env.py:204-304, 472-652
 #pragma once
+#include "../../include/llq.h"
 #include "llq_math.cuh"
 #include <cuda_pipeline.h>
 #include <stdint.h>
@@ -67,15 +68,15 @@ struct EnvArrays {      // SoA device arrays, N envs
   float* reward_sum;    // [N]
   int* episode_steps;   // [N]
   long long* episode;   // [N]
-  float* warm;          // [4][N]
-  float* obs;           // [N][207] (history carry)
+  float* warm;          // [LLQ_MAX_SPHERES][N]
+  float* obs;           // [N][obs width] (history carry)
   float* kin;           // [37][N]
   float* foot_pos;      // [12][N]
   float* done_reward;   // [N] reward_sum at termination
   unsigned char* done;  // [N]
   float* reward;        // [N]
   unsigned long long* counters;  // [8]
-  double* aux;          // [18][N] EPMC bookkeeping (include/llq.h LLQ_F_AUX)
+  double* aux;          // [LLQ_AUX_DIM][N] EPMC / SEPMC bookkeeping, slots LLQ_AUX_* (include/llq.h)
   int* ob_id;           // [N] active hurdle plate
   float* boxes;         // [N][36][6] EPMC corridor: centre xyz, half extents xyz (walls first)
   int* nbox;            // [N]
@@ -130,6 +131,38 @@ LLQ_DI V3 foot_in_base(const LegConst& L, float q1, float q2, float q3) {
   return p;
 }
 
+// Robot write-back shared by the step tail and the reset kernel: lane k stores its leg's joints and foot (world), lane 0 the base
+// (qb in the pybullet inertial-frame convention) and the clock.
+LLQ_DI void write_robot(const EnvArrays& E, int N, int env, int k, const float (&q)[3], const float (&qd)[3], V3 foot, double px, double py,
+                        double pz, Q4 qb, V3 lin, V3 ang, double time) {
+  float* sw = E.st;
+#pragma unroll
+  for (int t = 0; t < 3; t++) { sw[(10 + 3 * k + t) * N + env] = q[t]; sw[(22 + 3 * k + t) * N + env] = qd[t]; }
+  E.foot_pos[(3 * k) * N + env] = foot.x; E.foot_pos[(3 * k + 1) * N + env] = foot.y; E.foot_pos[(3 * k + 2) * N + env] = foot.z;
+  if (k == 0) {
+    E.pos[env] = px; E.pos[N + env] = py; E.pos[2 * N + env] = pz;
+    const float b[10] = {qb.x, qb.y, qb.z, qb.w, lin.x, lin.y, lin.z, ang.x, ang.y, ang.z};
+#pragma unroll
+    for (int t = 0; t < 10; t++) sw[t * N + env] = b[t];
+    E.time[env] = time;
+  }
+}
+// end of an env step (lane 0): reward, reward sum, step count, done; returns the new reward sum
+LLQ_DI float write_step(const EnvArrays& E, int env, float rew, bool done) {
+  const float rs = E.reward_sum[env] + rew;
+  E.reward_sum[env] = rs;
+  E.episode_steps[env] += 1;
+  E.reward[env] = rew;
+  E.done[env] = done ? 1 : 0;
+  return rs;
+}
+// start of an episode: no contact memory (lane k clears the warm start of spheres k, k + 4, ...); lane 0 resets the bookkeeping
+LLQ_DI void write_reset(const EnvArrays& E, int N, int env, int k, long long episode) {
+#pragma unroll
+  for (int t = 0; t < LLQ_MAX_SPHERES / 4; t++) E.warm[(4 * t + k) * N + env] = 0.f;
+  if (k == 0) { E.reward_sum[env] = 0.f; E.episode_steps[env] = 0; E.episode[env] = episode; }
+}
+
 // Philox4x32-10
 LLQ_DI void philox4x32_10(unsigned (&c)[4], unsigned k0, unsigned k1) {
 #pragma unroll
@@ -165,11 +198,6 @@ LLQ_DI void epmc_randomize_push(const StepParams& P, unsigned long long seed, lo
   pf[0] = (float)(h * cs); pf[1] = (float)(h * sn); pf[2] = (float)((double)P.pv_lo + u[2] * ((double)P.pv_hi - (double)P.pv_lo));
 }
 
-
-LLQ_DI void push_force_of_draw(const StepParams& P, unsigned long long seed, long long gid, long long ep, int index, float (&pf)[3]) {
-  int d = index;
-  epmc_randomize_push(P, seed, gid, ep, d, pf);
-}
 
 // ---------------------------------------------------------------------------------------------------------------
 // SEPMC (ChaseTagGameEnv, max_game/chase_tag_game_env.py = CTG; arena = max_game/bullet_static_entities.py:863-902):
@@ -239,15 +267,13 @@ LLQ_DI void leg_points(const ModelConst& M, const LegConst& L, int k, const floa
   f = rot<1>(f, c2, s2) + ld3(L.j[1].r);
   foot = rot<0>(f, c1, s1) + hip;
 }
-// force of push-randomiser draw `index` (PR:89-99)
 
 // staging row of SEPMC (kNewObs floats per robot): prop 33 | action 12 | R 9 (45) | pos 3 (54) | flag xy 2 (57) | yaw 1 (59) | pad 2 |
 // small vectors 52 (62): percept_vec 5, oppo_info 15, oppo_info_cheat 15, flag_info 7, flag_info_cheat 7, with_flag 2, control_spd 1
 struct PairState { int with_flag, flag_draws, visible, sw; double flag_x, flag_y; };
 
 // End-of-step pair logic shared by the step and the reset kernels (CTG:495-596, 472-493): visibility, flag switch, the small
-// observation vectors.  Every lane of both robots runs it; `snew` is the robot's staging row, `spart` the partner's.
-template <int PX = 4>   // lane distance of the partner robot: 4 (one robot = 4 lanes) or 16 (one robot = a half-warp)
+// observation vectors.  Every lane of both robots runs it; `snew` is the robot's staging row, `spart` the partner's (4 lanes away).
 LLQ_DI void sepmc_pair_tail(const ModelConst& M, const LegConst& L, int k, int robot, float* snew, const float* spart, double px, double py,
                             double pz, Q4 qp, Q4 qb, V3 vw, V3 ww, const float (&q)[3], bool touch_own, float fix_spd, unsigned long long seed,
                             long long pair_gid, long long epi, PairState& S) {
@@ -267,11 +293,11 @@ LLQ_DI void sepmc_pair_tail(const ModelConst& M, const LegConst& L, int k, int r
   }
   __syncwarp();
   // partner's root state
-  const double ox = __shfl_xor_sync(FULL, px, PX), oy = __shfl_xor_sync(FULL, py, PX), oz = __shfl_xor_sync(FULL, pz, PX);
-  const Q4 oq = Q4{__shfl_xor_sync(FULL, qb.x, PX), __shfl_xor_sync(FULL, qb.y, PX), __shfl_xor_sync(FULL, qb.z, PX), __shfl_xor_sync(FULL, qb.w, PX)};
-  const V3 ov = V3{__shfl_xor_sync(FULL, vw.x, PX), __shfl_xor_sync(FULL, vw.y, PX), __shfl_xor_sync(FULL, vw.z, PX)};
-  const V3 oww = V3{__shfl_xor_sync(FULL, ww.x, PX), __shfl_xor_sync(FULL, ww.y, PX), __shfl_xor_sync(FULL, ww.z, PX)};
-  const bool touch_other = __shfl_xor_sync(FULL, touch_own ? 1 : 0, PX) != 0;
+  const double ox = __shfl_xor_sync(FULL, px, 4), oy = __shfl_xor_sync(FULL, py, 4), oz = __shfl_xor_sync(FULL, pz, 4);
+  const Q4 oq = Q4{__shfl_xor_sync(FULL, qb.x, 4), __shfl_xor_sync(FULL, qb.y, 4), __shfl_xor_sync(FULL, qb.z, 4), __shfl_xor_sync(FULL, qb.w, 4)};
+  const V3 ov = V3{__shfl_xor_sync(FULL, vw.x, 4), __shfl_xor_sync(FULL, vw.y, 4), __shfl_xor_sync(FULL, vw.z, 4)};
+  const V3 oww = V3{__shfl_xor_sync(FULL, ww.x, 4), __shfl_xor_sync(FULL, ww.y, 4), __shfl_xor_sync(FULL, ww.z, 4)};
+  const bool touch_other = __shfl_xor_sync(FULL, touch_own ? 1 : 0, 4) != 0;
   const V3 opos = V3{(float)ox, (float)oy, (float)oz};
   const float fx = (float)S.flag_x, fy = (float)S.flag_y;
   // visibility (CTG:472-493): the root segment is cast from robot 0 to robot 1 for both agents
@@ -672,17 +698,18 @@ struct ResetParams {
   int update_table;                           // 1 after a step
 };
 
-template <int BLOCK, int ENV>
-__global__ void __launch_bounds__(BLOCK) pmc_reset_kernel(EnvArrays E, MocapDev mc, StepParams P, const ModelConst* __restrict__ gmodel,
-                                                          ResetParams RP, float* obs2, long long obs2_ld) {
+constexpr int kResetBlock = 128;
+template <int ENV>
+__global__ void __launch_bounds__(kResetBlock) pmc_reset_kernel(EnvArrays E, MocapDev mc, StepParams P, const ModelConst* __restrict__ gmodel,
+                                                                ResetParams RP, float* obs2, long long obs2_ld) {
   extern __shared__ double s_cdf[];            // [n_clips]
   __shared__ __align__(16) ModelConst M;
-  __shared__ __align__(16) float s_new[BLOCK / 4][kNewObs];
-  prefetch_model(gmodel, &M, BLOCK);
+  __shared__ __align__(16) float s_new[kResetBlock / 4][kNewObs];
+  prefetch_model(gmodel, &M, kResetBlock);
   __pipeline_commit();
   const int C = mc.n_clips;
   // ---- prioritized sampling table: every block recomputes it identically; block 0 publishes it
-  for (int c = threadIdx.x; c < C; c += BLOCK) {
+  for (int c = threadIdx.x; c < C; c += kResetBlock) {
     double avg = RP.avg_old[c];
     if (RP.update_table) {
       int w = RP.winner_cur[c];
@@ -692,9 +719,9 @@ __global__ void __launch_bounds__(BLOCK) pmc_reset_kernel(EnvArrays E, MocapDev 
   }
   __syncthreads();
   if (RP.update_table && blockIdx.x == 0)
-    for (int c = threadIdx.x; c < C; c += BLOCK) { RP.avg_new[c] = s_cdf[c]; RP.winner_next[c] = -1; }
+    for (int c = threadIdx.x; c < C; c += kResetBlock) { RP.avg_new[c] = s_cdf[c]; RP.winner_next[c] = -1; }
   __syncthreads();
-  for (int c = threadIdx.x; c < C; c += BLOCK) s_cdf[c] = pow(1.0 - s_cdf[c], RP.factor);
+  for (int c = threadIdx.x; c < C; c += kResetBlock) s_cdf[c] = pow(1.0 - s_cdf[c], RP.factor);
   __syncthreads();
   // p = w / sum(w), cdf = cumsum(p) / cumsum(p)[-1] exactly as np.random.choice builds them: the two sums run sequentially on one
   // thread (their order fixes the last bits), the 2 C fp64 divisions -- 3/4 of this section's latency when thread 0 did them one
@@ -706,7 +733,7 @@ __global__ void __launch_bounds__(BLOCK) pmc_reset_kernel(EnvArrays E, MocapDev 
     s_tot = tot;
   }
   __syncthreads();
-  for (int c = threadIdx.x; c < C; c += BLOCK) {
+  for (int c = threadIdx.x; c < C; c += kResetBlock) {
     const double pc = s_cdf[c] / s_tot;
     s_cdf[c] = pc;
     if (blockIdx.x == 0) RP.prob[c] = pc;
@@ -718,13 +745,13 @@ __global__ void __launch_bounds__(BLOCK) pmc_reset_kernel(EnvArrays E, MocapDev 
     s_tot = s_cdf[C - 1];
   }
   __syncthreads();
-  for (int c = threadIdx.x; c < C; c += BLOCK) s_cdf[c] = s_cdf[c] / s_tot;
+  for (int c = threadIdx.x; c < C; c += kResetBlock) s_cdf[c] = s_cdf[c] / s_tot;
   __syncthreads();
 
   __pipeline_wait_prior(0);
   __syncthreads();
   const int N = P.n_envs;
-  const int gtid = blockIdx.x * BLOCK + threadIdx.x;
+  const int gtid = blockIdx.x * kResetBlock + threadIdx.x;
   const int env_raw = gtid >> 2;
   const int env = env_raw < N ? env_raw : N - 1;
   const bool valid = env_raw < N;
@@ -752,7 +779,7 @@ __global__ void __launch_bounds__(BLOCK) pmc_reset_kernel(EnvArrays E, MocapDev 
     const double foot_mu = (double)P.fr_lo + u0[2] * ((double)P.fr_hi - (double)P.fr_lo);
     const double px = robot == 0 ? -2.0 + 4.0 * u0[3] : -2.0 + 4.0 * u1[1], py = robot == 0 ? -2.0 + 4.0 * u1[0] : -2.0 + 4.0 * u1[2];
     // both robots are handed the same mutable init dict => one running yaw for the pair (CTG:209-215)
-    const double acc0 = E.aux[16 * N + (env & ~1)];
+    const double acc0 = E.aux[LLQ_AUX_YAW_ACCUM_DEG * N + (env & ~1)];
     const double yaw_a = fmod(acc0 + 360.0 * u1[3], 360.0), yaw_b = fmod(yaw_a + 360.0 * u2[0], 360.0);
     const double yaw_deg = robot == 0 ? yaw_a : yaw_b;
     double sn, cs;
@@ -767,7 +794,7 @@ __global__ void __launch_bounds__(BLOCK) pmc_reset_kernel(EnvArrays E, MocapDev 
     const Q4 qp = qmul(qnormalize(qn), qconj(qI));
     PairState PS = {robot == 0 ? wflag : 1 - wflag, 0, 1, 0, -2.0 + 4.0 * u2[1], -2.0 + 4.0 * u2[2]};
     // reset() runs _prepare_drill too (CTG:302): its flag-switch test reads the stale manifolds of the previous episode's last step
-    const bool touch_own = E.aux[17 * N + env] != 0.0;
+    const bool touch_own = E.aux[LLQ_AUX_FLAG_TOUCH * N + env] != 0.0;
     float* snew = &s_new[threadIdx.x >> 2][0];
     const float* spart = &s_new[(threadIdx.x >> 2) ^ 1][0];
     sepmc_pair_tail(M, L, k, robot, snew, spart, px, py, 0.5, qp, qn, lin, ang, q, touch_own, fix_spd, RP.seed, gid, ep, PS);
@@ -777,23 +804,18 @@ __global__ void __launch_bounds__(BLOCK) pmc_reset_kernel(EnvArrays E, MocapDev 
     float pf[3] = {0.f, 0.f, 0.f};
     if (P.push_enabled) push_draws = 1;                              // PR:52-54: draw #0 becomes the current _randomized_force
     if (doit) {
-      float* sw = E.st;
       V3 f = mul(qmat(qp), foot_in_base(L, q[0], q[1], q[2]));
-#pragma unroll
-      for (int i = 0; i < 3; i++) { sw[(10 + 3 * k + i) * N + env] = q[i]; sw[(22 + 3 * k + i) * N + env] = qd[i]; }
-      E.warm[k * N + env] = 0.f;
-      E.foot_pos[(3 * k) * N + env] = (float)px + f.x; E.foot_pos[(3 * k + 1) * N + env] = (float)py + f.y; E.foot_pos[(3 * k + 2) * N + env] = 0.5f + f.z;
+      write_robot(E, N, env, k, q, qd, V3{(float)px + f.x, (float)py + f.y, 0.5f + f.z}, px, py, 0.5, qn, lin, ang, 0.0);
+      write_reset(E, N, env, k, ep + 1);
       if (k == 0) {
-        E.pos[env] = px; E.pos[N + env] = py; E.pos[2 * N + env] = 0.5;
-        float b[10] = {qn.x, qn.y, qn.z, qn.w, lin.x, lin.y, lin.z, ang.x, ang.y, ang.z};
-#pragma unroll
-        for (int i = 0; i < 10; i++) sw[i * N + env] = b[i];
-        E.time[env] = 0.0; E.reward_sum[env] = 0.f; E.episode_steps[env] = 0; E.episode[env] = ep + 1;
         double* A = E.aux;
-        A[env] = 0; A[N + env] = PS.with_flag; A[2 * N + env] = PS.flag_x; A[3 * N + env] = PS.flag_y; A[4 * N + env] = fix_spd;
-        A[5 * N + env] = PS.visible; A[6 * N + env] = PS.sw; A[7 * N + env] = 0.0; A[8 * N + env] = 0.0; A[9 * N + env] = P.push_start_count;
-        A[10 * N + env] = pf[0]; A[11 * N + env] = pf[1]; A[12 * N + env] = pf[2]; A[13 * N + env] = foot_mu; A[14 * N + env] = push_draws;
-        A[15 * N + env] = PS.flag_draws; A[16 * N + env] = yaw_b; A[17 * N + env] = touch_own ? 1.0 : 0.0;
+        A[LLQ_AUX_COUNTER * N + env] = 0; A[LLQ_AUX_WITH_FLAG * N + env] = PS.with_flag; A[LLQ_AUX_FLAG_X * N + env] = PS.flag_x;
+        A[LLQ_AUX_FLAG_Y * N + env] = PS.flag_y; A[LLQ_AUX_CONTROL_SPD * N + env] = fix_spd;
+        A[LLQ_AUX_OPPO_VISIBLE * N + env] = PS.visible; A[LLQ_AUX_SWITCH_FLAG * N + env] = PS.sw; A[LLQ_AUX_TOTAL_SPD * N + env] = 0.0;
+        A[LLQ_AUX_MAX_SPD * N + env] = 0.0; A[LLQ_AUX_PUSH_COUNT * N + env] = P.push_start_count;
+        A[LLQ_AUX_PUSH_F * N + env] = pf[0]; A[(LLQ_AUX_PUSH_F + 1) * N + env] = pf[1]; A[(LLQ_AUX_PUSH_F + 2) * N + env] = pf[2];
+        A[LLQ_AUX_FOOT_FRICTION * N + env] = foot_mu; A[LLQ_AUX_PUSH_DRAWS * N + env] = push_draws;
+        A[LLQ_AUX_FLAG_DRAWS * N + env] = PS.flag_draws; A[LLQ_AUX_YAW_ACCUM_DEG * N + env] = yaw_b; A[LLQ_AUX_FLAG_TOUCH * N + env] = touch_own ? 1.0 : 0.0;
       }
     }
   } else if (ENV == 1 || ENV == 3) {
@@ -807,7 +829,7 @@ __global__ void __launch_bounds__(BLOCK) pmc_reset_kernel(EnvArrays E, MocapDev 
     float pf[3] = {0.f, 0.f, 0.f};
     if (P.push_enabled) epmc_randomize_push(P, RP.seed, gid, ep, push_draws, pf);                          // PR:52-54
     const int cmd_freq = P.cmd_freq_lo + (int)floor(u[2] * (double)(P.cmd_freq_hi - P.cmd_freq_lo));       // PGE:223
-    const double yaw_deg = fmod(E.aux[16 * N + env] + 360.0 * u[1], 360.0);                                // PGE:181-189 (accumulates)
+    const double yaw_deg = fmod(E.aux[LLQ_AUX_YAW_ACCUM_DEG * N + env] + 360.0 * u[1], 360.0);                                // PGE:181-189 (accumulates)
     double sn, cs;
     sincos(0.5 * yaw_deg * (3.14159265358979323846 / 180.0), &sn, &cs);
     const float* I0 = M.init_state;
@@ -818,7 +840,7 @@ __global__ void __launch_bounds__(BLOCK) pmc_reset_kernel(EnvArrays E, MocapDev 
     const V3 lin = V3{I0[7], I0[8], I0[9]}, ang = V3{I0[10], I0[11], I0[12]};
     float* snew = &s_new[threadIdx.x >> 2][0];
     const M3 Rq = qmat(qnormalize(qn));
-    const float target_spd = (float)E.aux[4 * N + env];            // persists across episodes (PGE:170-172)
+    const float target_spd = (float)E.aux[LLQ_AUX_TARGET_SPD * N + env];            // persists across episodes (PGE:170-172)
     double tgx0 = 8.0;
     int nb0 = 0;
     if (ENV == 3) nb0 = generate_corridor(P, RP.seed, gid, ep, E.boxes + (size_t)env * (6 * kMaxBoxes), doit && k == 0, tgx0);   // PGE:216-219
@@ -841,93 +863,80 @@ __global__ void __launch_bounds__(BLOCK) pmc_reset_kernel(EnvArrays E, MocapDev 
       stage_corridor_masks(snew, E.boxes + (size_t)env * (6 * kMaxBoxes), doit ? nb0 : E.nbox[env], k, 0.f, 0.f, 0.5f, atan2f(Rq.a10, Rq.a00));
     }
     if (doit) {
-      float* sw = E.st;
       const Q4 qI = Q4{M.base.qI[0], M.base.qI[1], M.base.qI[2], M.base.qI[3]};
       V3 f = mul(qmat(qmul(qnormalize(qn), qconj(qI))), foot_in_base(L, q[0], q[1], q[2]));
-#pragma unroll
-      for (int i = 0; i < 3; i++) { sw[(10 + 3 * k + i) * N + env] = q[i]; sw[(22 + 3 * k + i) * N + env] = qd[i]; }
-      E.warm[k * N + env] = 0.f;
-      E.foot_pos[(3 * k) * N + env] = f.x; E.foot_pos[(3 * k + 1) * N + env] = f.y; E.foot_pos[(3 * k + 2) * N + env] = 0.5f + f.z;
+      write_robot(E, N, env, k, q, qd, V3{f.x, f.y, 0.5f + f.z}, 0.0, 0.0, 0.5, qn, lin, ang, 0.0);
+      write_reset(E, N, env, k, ep + 1);
       if (k == 0) {
-        E.pos[env] = 0.0; E.pos[N + env] = 0.0; E.pos[2 * N + env] = 0.5;
-        float b[10] = {qn.x, qn.y, qn.z, qn.w, lin.x, lin.y, lin.z, ang.x, ang.y, ang.z};
-#pragma unroll
-        for (int i = 0; i < 10; i++) sw[i * N + env] = b[i];
-        E.time[env] = 0.0; E.reward_sum[env] = 0.f; E.episode_steps[env] = 0; E.episode[env] = ep + 1;
         double* A = E.aux;
-        A[env] = 0; A[N + env] = cmd_freq; A[2 * N + env] = tgx0; A[3 * N + env] = 0.0; A[6 * N + env] = fabs(tgx0); A[7 * N + env] = 0.0;
-        A[17 * N + env] = fabs(tgx0);                                  // init_pos_diff_len (PGE:192-195)
+        A[LLQ_AUX_COUNTER * N + env] = 0; A[LLQ_AUX_CMD_FREQ * N + env] = cmd_freq; A[LLQ_AUX_TARGET_X * N + env] = tgx0;
+        A[LLQ_AUX_TARGET_Y * N + env] = 0.0; A[LLQ_AUX_LAST_POS_DIFF_LEN * N + env] = fabs(tgx0); A[LLQ_AUX_TOTAL_SPD * N + env] = 0.0;
+        A[LLQ_AUX_INIT_POS_DIFF_LEN * N + env] = fabs(tgx0);                                  // init_pos_diff_len (PGE:192-195)
         if (ENV == 3) E.nbox[env] = nb0;
-        A[8 * N + env] = 0.0; A[9 * N + env] = P.push_start_count; A[10 * N + env] = pf[0]; A[11 * N + env] = pf[1]; A[12 * N + env] = pf[2];
-        A[13 * N + env] = foot_mu; A[14 * N + env] = push_draws; A[15 * N + env] = 0; A[16 * N + env] = yaw_deg;
+        A[LLQ_AUX_MAX_SPD * N + env] = 0.0; A[LLQ_AUX_PUSH_COUNT * N + env] = P.push_start_count; A[LLQ_AUX_PUSH_F * N + env] = pf[0];
+        A[(LLQ_AUX_PUSH_F + 1) * N + env] = pf[1]; A[(LLQ_AUX_PUSH_F + 2) * N + env] = pf[2];
+        A[LLQ_AUX_FOOT_FRICTION * N + env] = foot_mu; A[LLQ_AUX_PUSH_DRAWS * N + env] = push_draws; A[LLQ_AUX_CMD_DRAWS * N + env] = 0;
+        A[LLQ_AUX_YAW_ACCUM_DEG * N + env] = yaw_deg;
       }
     }
   } else {
-  int clip; double t0;
-  long long ep = E.episode[env];
-  if (RP.mode == 2) {
-    clip = RP.clip_in[env]; t0 = RP.time_in[env];
-    if (!doit) { clip = 0; t0 = 0.0; }     // entries of masked-out envs are not validated by the host: never index the table with them
-  } else {
-    long long gid = RP.gid0 + env;
-    unsigned c4[4] = {(unsigned)gid, (unsigned)((unsigned long long)gid >> 32), (unsigned)ep, (unsigned)((unsigned long long)ep >> 32)};
-    philox4x32_10(c4, (unsigned)RP.seed, (unsigned)(RP.seed >> 32));
-    double u1 = ((double)c4[0] + 0.5) * (1.0 / 4294967296.0), u2 = ((double)c4[1] + 0.5) * (1.0 / 4294967296.0);
-    clip = C - 1;
-    for (int c = 0; c < C; c++) if (s_cdf[c] > u1) { clip = c; break; }
-    int nf = mc.clip_off[clip + 1] - mc.clip_off[clip];
-    t0 = u2 * (P.frame_dt * (double)(nf - P.margin - 1));
-    ep += 1;
-  }
-  int frame_id = (int)floor(t0 / P.frame_dt);
-  double frac = (t0 - frame_id * P.frame_dt) / P.frame_dt;
-  {
-    const int last = mc.clip_off[clip + 1] - mc.clip_off[clip] - P.margin + 2;
-    if (frame_id > last) { frame_id = last; frac = 0.0; }
-    if (frame_id < 0) { frame_id = 0; frac = 0.0; }
-  }
-  const MocapFrame* f0 = mc.frames + mc.clip_off[clip] + frame_id;
-  KinBase kb = mocap_base(f0, f0 + 1, frac, P.frame_dt);
-  float inv = (float)(1.0 / P.frame_dt), fr = (float)frac;
-  float q[3], qd[3];
-#pragma unroll
-  for (int i = 0; i < 3; i++) {
-    float c = f0->q[3 * k + i], n = f0[1].q[3 * k + i];
-    q[i] = fmaf(fr, n - c, c);
-    qd[i] = (n - c) * inv;
-  }
-  float* snew = &s_new[threadIdx.x >> 2][0];
-  build_obs_new(mc, P, M, k, clip, frame_id, frac, kb.px, kb.py, kb.pz, kb.q, kb.lin, kb.ang, q, qd, snew);
-  if (doit) {
-    float* sw = E.st;
-    const Q4 qI = Q4{M.base.qI[0], M.base.qI[1], M.base.qI[2], M.base.qI[3]};
-    V3 f = mul(qmat(qmul(qnormalize(kb.q), qconj(qI))), foot_in_base(L, q[0], q[1], q[2]));
+    int clip; double t0;
+    long long ep = E.episode[env];
+    if (RP.mode == 2) {
+      clip = RP.clip_in[env]; t0 = RP.time_in[env];
+      if (!doit) { clip = 0; t0 = 0.0; }     // entries of masked-out envs are not validated by the host: never index the table with them
+    } else {
+      long long gid = RP.gid0 + env;
+      unsigned c4[4] = {(unsigned)gid, (unsigned)((unsigned long long)gid >> 32), (unsigned)ep, (unsigned)((unsigned long long)ep >> 32)};
+      philox4x32_10(c4, (unsigned)RP.seed, (unsigned)(RP.seed >> 32));
+      double u1 = ((double)c4[0] + 0.5) * (1.0 / 4294967296.0), u2 = ((double)c4[1] + 0.5) * (1.0 / 4294967296.0);
+      clip = C - 1;
+      for (int c = 0; c < C; c++) if (s_cdf[c] > u1) { clip = c; break; }
+      int nf = mc.clip_off[clip + 1] - mc.clip_off[clip];
+      t0 = u2 * (P.frame_dt * (double)(nf - P.margin - 1));
+      ep += 1;
+    }
+    int frame_id = (int)floor(t0 / P.frame_dt);
+    double frac = (t0 - frame_id * P.frame_dt) / P.frame_dt;
+    {
+      const int last = mc.clip_off[clip + 1] - mc.clip_off[clip] - P.margin + 2;
+      if (frame_id > last) { frame_id = last; frac = 0.0; }
+      if (frame_id < 0) { frame_id = 0; frac = 0.0; }
+    }
+    const MocapFrame* f0 = mc.frames + mc.clip_off[clip] + frame_id;
+    KinBase kb = mocap_base(f0, f0 + 1, frac, P.frame_dt);
+    float inv = (float)(1.0 / P.frame_dt), fr = (float)frac;
+    float q[3], qd[3];
 #pragma unroll
     for (int i = 0; i < 3; i++) {
-      sw[(10 + 3 * k + i) * N + env] = q[i]; sw[(22 + 3 * k + i) * N + env] = qd[i];
-      E.kin[(13 + 3 * k + i) * N + env] = q[i]; E.kin[(25 + 3 * k + i) * N + env] = qd[i];
+      float c = f0->q[3 * k + i], n = f0[1].q[3 * k + i];
+      q[i] = fmaf(fr, n - c, c);
+      qd[i] = (n - c) * inv;
     }
-    E.warm[k * N + env] = 0.f;
-    E.foot_pos[(3 * k) * N + env] = (float)kb.px + f.x; E.foot_pos[(3 * k + 1) * N + env] = (float)kb.py + f.y;
-    E.foot_pos[(3 * k + 2) * N + env] = (float)kb.pz + f.z;
-    if (k == 0) {
-      E.pos[env] = kb.px; E.pos[N + env] = kb.py; E.pos[2 * N + env] = kb.pz;
-      float b[13] = {kb.q.x, kb.q.y, kb.q.z, kb.q.w, kb.lin.x, kb.lin.y, kb.lin.z, kb.ang.x, kb.ang.y, kb.ang.z, 0.f, 0.f, 0.f};
+    float* snew = &s_new[threadIdx.x >> 2][0];
+    build_obs_new(mc, P, M, k, clip, frame_id, frac, kb.px, kb.py, kb.pz, kb.q, kb.lin, kb.ang, q, qd, snew);
+    if (doit) {
+      const Q4 qI = Q4{M.base.qI[0], M.base.qI[1], M.base.qI[2], M.base.qI[3]};
+      V3 f = mul(qmat(qmul(qnormalize(kb.q), qconj(qI))), foot_in_base(L, q[0], q[1], q[2]));
+      write_robot(E, N, env, k, q, qd, V3{(float)kb.px + f.x, (float)kb.py + f.y, (float)kb.pz + f.z}, kb.px, kb.py, kb.pz, kb.q, kb.lin, kb.ang, t0);
+      write_reset(E, N, env, k, ep);
 #pragma unroll
-      for (int i = 0; i < 10; i++) sw[i * N + env] = b[i];
-      E.kin[env] = (float)kb.px; E.kin[N + env] = (float)kb.py; E.kin[2 * N + env] = (float)kb.pz;
+      for (int i = 0; i < 3; i++) { E.kin[(13 + 3 * k + i) * N + env] = q[i]; E.kin[(25 + 3 * k + i) * N + env] = qd[i]; }
+      if (k == 0) {
+        const float b[10] = {kb.q.x, kb.q.y, kb.q.z, kb.q.w, kb.lin.x, kb.lin.y, kb.lin.z, kb.ang.x, kb.ang.y, kb.ang.z};
+        E.kin[env] = (float)kb.px; E.kin[N + env] = (float)kb.py; E.kin[2 * N + env] = (float)kb.pz;
 #pragma unroll
-      for (int i = 0; i < 10; i++) E.kin[(3 + i) * N + env] = b[i];
-      E.time[env] = t0; E.clip[env] = clip; E.reward_sum[env] = 0.f; E.episode_steps[env] = 0; E.episode[env] = ep;
-      E.ob_id[env] = 0;                                            // PLE:179
+        for (int i = 0; i < 10; i++) E.kin[(3 + i) * N + env] = b[i];
+        E.clip[env] = clip;
+        E.ob_id[env] = 0;                                            // PLE:179
+      }
     }
-  }
   }
   __syncwarp();
   unsigned rows = 0;
 #pragma unroll
   for (int e = 0; e < 8; e++) if ((wm >> (4 * e)) & 1u) rows |= 1u << e;
-  const int warp_env0 = (blockIdx.x * BLOCK + (threadIdx.x & ~31)) >> 2;
+  const int warp_env0 = (blockIdx.x * kResetBlock + (threadIdx.x & ~31)) >> 2;
   emit_obs_rows<ENV>(E.obs, obs2, obs2_ld, &s_new[(threadIdx.x & ~31) >> 2][0], &s_new[0][0], warp_env0, N, 1, rows, E.boxes);
 }
 

@@ -514,27 +514,12 @@ LLQ_DI void step_tail(const EnvArrays& E, const MocapDev& mc, const StepParams& 
     done = fall || ended || diff || ob_hit || bad;                                     // PLE:347
     rew_out = rew;
     if (wr) {
-      float* sw = E.st;
+      write_robot(E, N, env, k, q, qd, fd, px, py, pz, qb, vw, ww, time);
 #pragma unroll
-      for (int t = 0; t < 3; t++) {
-        sw[(10 + 3 * k + t) * N + env] = q[t];
-        sw[(22 + 3 * k + t) * N + env] = qd[t];
-        E.kin[(13 + 3 * k + t) * N + env] = oc.kq[t];
-        E.kin[(25 + 3 * k + t) * N + env] = oc.kqd[t];
-      }
-      E.foot_pos[(3 * k) * N + env] = fd.x; E.foot_pos[(3 * k + 1) * N + env] = fd.y; E.foot_pos[(3 * k + 2) * N + env] = fd.z;
+      for (int t = 0; t < 3; t++) { E.kin[(13 + 3 * k + t) * N + env] = oc.kq[t]; E.kin[(25 + 3 * k + t) * N + env] = oc.kqd[t]; }
       if (k == 0) {
-        E.pos[env] = px; E.pos[N + env] = py; E.pos[2 * N + env] = pz;
-        sw[env] = qb.x; sw[N + env] = qb.y; sw[2 * N + env] = qb.z; sw[3 * N + env] = qb.w;
-        sw[4 * N + env] = vw.x; sw[5 * N + env] = vw.y; sw[6 * N + env] = vw.z;
-        sw[7 * N + env] = ww.x; sw[8 * N + env] = ww.y; sw[9 * N + env] = ww.z;
-        E.time[env] = time;
         if (P.has_ob) E.ob_id[env] = ob_id;
-        float rs = E.reward_sum[env] + rew;
-        E.reward_sum[env] = rs;
-        E.episode_steps[env] += 1;
-        E.reward[env] = rew;
-        E.done[env] = done ? 1 : 0;
+        const float rs = write_step(E, env, rew, done);
         E.kin[env] = (float)oc.kb.px; E.kin[N + env] = (float)oc.kb.py; E.kin[2 * N + env] = (float)oc.kb.pz;
         E.kin[3 * N + env] = oc.kb.q.x; E.kin[4 * N + env] = oc.kb.q.y; E.kin[5 * N + env] = oc.kb.q.z; E.kin[6 * N + env] = oc.kb.q.w;
         E.kin[7 * N + env] = oc.kb.lin.x; E.kin[8 * N + env] = oc.kb.lin.y; E.kin[9 * N + env] = oc.kb.lin.z;
@@ -548,15 +533,15 @@ LLQ_DI void step_tail(const EnvArrays& E, const MocapDev& mc, const StepParams& 
   } else if (ENV == 2) {
     // ---------------- SEPMC tail (CTG:378-424, 458-470, 495-596, 640-652)
     const double* A = E.aux;
-    int counter = (int)A[env];
-    PS.with_flag = (int)A[N + env]; PS.flag_x = A[2 * N + env]; PS.flag_y = A[3 * N + env];
-    const float fix_spd = (float)A[4 * N + env];
-    double total_spd = A[7 * N + env], max_spd = A[8 * N + env];
-    PS.flag_draws = (int)A[15 * N + env];
+    int counter = (int)A[LLQ_AUX_COUNTER * N + env];
+    PS.with_flag = (int)A[LLQ_AUX_WITH_FLAG * N + env]; PS.flag_x = A[LLQ_AUX_FLAG_X * N + env]; PS.flag_y = A[LLQ_AUX_FLAG_Y * N + env];
+    const float fix_spd = (float)A[LLQ_AUX_CONTROL_SPD * N + env];
+    double total_spd = A[LLQ_AUX_TOTAL_SPD * N + env], max_spd = A[LLQ_AUX_MAX_SPD * N + env];
+    PS.flag_draws = (int)A[LLQ_AUX_FLAG_DRAWS * N + env];
     qb = qmul(qp, qI);
     float* snew = s_new + el * kNewObs;
     const float* spart = s_new + (el ^ 1) * kNewObs;
-    sepmc_pair_tail<4>(M, L, k, robot, snew, spart, px, py, pz, qp, qb, vw, ww, q, touch_own, fix_spd, seed, pair_gid, epi, PS);
+    sepmc_pair_tail(M, L, k, robot, snew, spart, px, py, pz, qp, qb, vw, ww, q, touch_own, fix_spd, seed, pair_gid, epi, PS);
 #pragma unroll
     for (int t = 0; t < 3; t++) { snew[3 * k + t] = q[t]; snew[12 + 3 * k + t] = qd[t]; snew[kPropDim + 3 * k + t] = act_src[3 * k + t]; }
     const float spd = sqrtf(vw.x * vw.x + vw.y * vw.y);              // stat_spd (CTG:368-373)
@@ -582,36 +567,27 @@ LLQ_DI void step_tail(const EnvArrays& E, const MocapDev& mc, const StepParams& 
       fd = V3{(float)px + f.x, (float)py + f.y, (float)pz + f.z};
     }
     if (wr) {
-      float* sw = E.st;
-#pragma unroll
-      for (int t = 0; t < 3; t++) { sw[(10 + 3 * k + t) * N + env] = q[t]; sw[(22 + 3 * k + t) * N + env] = qd[t]; }
-      E.foot_pos[(3 * k) * N + env] = fd.x; E.foot_pos[(3 * k + 1) * N + env] = fd.y; E.foot_pos[(3 * k + 2) * N + env] = fd.z;
+      write_robot(E, N, env, k, q, qd, fd, px, py, pz, qb, vw, ww, time);
       if (k == 0) {
-        E.pos[env] = px; E.pos[N + env] = py; E.pos[2 * N + env] = pz;
-        sw[env] = qb.x; sw[N + env] = qb.y; sw[2 * N + env] = qb.z; sw[3 * N + env] = qb.w;
-        sw[4 * N + env] = vw.x; sw[5 * N + env] = vw.y; sw[6 * N + env] = vw.z;
-        sw[7 * N + env] = ww.x; sw[8 * N + env] = ww.y; sw[9 * N + env] = ww.z;
-        E.time[env] = time;
-        E.reward_sum[env] += rew;
-        E.episode_steps[env] += 1;
-        E.reward[env] = rew;
-        E.done[env] = done ? 1 : 0;
+        write_step(E, env, rew, done);
         double* Aw = E.aux;
-        Aw[env] = counter; Aw[N + env] = PS.with_flag; Aw[2 * N + env] = PS.flag_x; Aw[3 * N + env] = PS.flag_y; Aw[5 * N + env] = PS.visible;
-        Aw[6 * N + env] = PS.sw; Aw[7 * N + env] = total_spd; Aw[8 * N + env] = max_spd; Aw[9 * N + env] = push_count;
-        Aw[10 * N + env] = pf[0]; Aw[11 * N + env] = pf[1]; Aw[12 * N + env] = pf[2]; Aw[14 * N + env] = push_draws; Aw[15 * N + env] = PS.flag_draws;
-        Aw[17 * N + env] = touch_own ? 1.0 : 0.0;
+        Aw[LLQ_AUX_COUNTER * N + env] = counter; Aw[LLQ_AUX_WITH_FLAG * N + env] = PS.with_flag; Aw[LLQ_AUX_FLAG_X * N + env] = PS.flag_x;
+        Aw[LLQ_AUX_FLAG_Y * N + env] = PS.flag_y; Aw[LLQ_AUX_OPPO_VISIBLE * N + env] = PS.visible;
+        Aw[LLQ_AUX_SWITCH_FLAG * N + env] = PS.sw; Aw[LLQ_AUX_TOTAL_SPD * N + env] = total_spd; Aw[LLQ_AUX_MAX_SPD * N + env] = max_spd;
+        Aw[LLQ_AUX_PUSH_COUNT * N + env] = push_count; Aw[LLQ_AUX_PUSH_F * N + env] = pf[0]; Aw[(LLQ_AUX_PUSH_F + 1) * N + env] = pf[1]; Aw[(LLQ_AUX_PUSH_F + 2) * N + env] = pf[2];
+        Aw[LLQ_AUX_PUSH_DRAWS * N + env] = push_draws; Aw[LLQ_AUX_FLAG_DRAWS * N + env] = PS.flag_draws; Aw[LLQ_AUX_FLAG_TOUCH * N + env] = touch_own ? 1.0 : 0.0;
       }
     }
   } else {
     // ---------------- EPMC tail (PGE:302-321, 334-358, 360-372, 479-539)
     const double* A = E.aux;
-    int counter = (int)A[env], cmd_draws = (int)A[15 * N + env];
-    const int cmd_freq = (int)A[N + env];
-    double tgx = A[2 * N + env], tgy = A[3 * N + env], target_angle = A[5 * N + env], last_len = A[6 * N + env];
-    double total_spd = A[7 * N + env], max_spd = A[8 * N + env];
-    float target_spd = (float)A[4 * N + env];
-    const double init_len = ENV == 3 ? A[17 * N + env] : 1.0;
+    int counter = (int)A[LLQ_AUX_COUNTER * N + env], cmd_draws = (int)A[LLQ_AUX_CMD_DRAWS * N + env];
+    const int cmd_freq = (int)A[LLQ_AUX_CMD_FREQ * N + env];
+    double tgx = A[LLQ_AUX_TARGET_X * N + env], tgy = A[LLQ_AUX_TARGET_Y * N + env];
+    double target_angle = A[LLQ_AUX_TARGET_ANGLE * N + env], last_len = A[LLQ_AUX_LAST_POS_DIFF_LEN * N + env];
+    double total_spd = A[LLQ_AUX_TOTAL_SPD * N + env], max_spd = A[LLQ_AUX_MAX_SPD * N + env];
+    float target_spd = (float)A[LLQ_AUX_TARGET_SPD * N + env];
+    const double init_len = ENV == 3 ? A[LLQ_AUX_INIT_POS_DIFF_LEN * N + env] : 1.0;
     {
       // the command of this step was drawn from the pose at the START of the step (PGE:302-317): recover it from the stored state
       const double sx0 = E.pos[env], sy0 = E.pos[N + env];
@@ -679,25 +655,16 @@ LLQ_DI void step_tail(const EnvArrays& E, const MocapDev& mc, const StepParams& 
       fd = V3{(float)px + f.x, (float)py + f.y, (float)pz + f.z};
     }
     if (wr) {
-      float* sw = E.st;
-#pragma unroll
-      for (int t = 0; t < 3; t++) { sw[(10 + 3 * k + t) * N + env] = q[t]; sw[(22 + 3 * k + t) * N + env] = qd[t]; }
-      E.foot_pos[(3 * k) * N + env] = fd.x; E.foot_pos[(3 * k + 1) * N + env] = fd.y; E.foot_pos[(3 * k + 2) * N + env] = fd.z;
+      write_robot(E, N, env, k, q, qd, fd, px, py, pz, qb, vw, ww, time);
       if (k == 0) {
-        E.pos[env] = px; E.pos[N + env] = py; E.pos[2 * N + env] = pz;
-        sw[env] = qb.x; sw[N + env] = qb.y; sw[2 * N + env] = qb.z; sw[3 * N + env] = qb.w;
-        sw[4 * N + env] = vw.x; sw[5 * N + env] = vw.y; sw[6 * N + env] = vw.z;
-        sw[7 * N + env] = ww.x; sw[8 * N + env] = ww.y; sw[9 * N + env] = ww.z;
-        E.time[env] = time;
-        E.reward_sum[env] += rew;
-        E.episode_steps[env] += 1;
-        E.reward[env] = rew;
-        E.done[env] = done ? 1 : 0;
+        write_step(E, env, rew, done);
         double* Aw = E.aux;
-        Aw[env] = counter; Aw[N + env] = cmd_freq; Aw[2 * N + env] = tgx; Aw[3 * N + env] = tgy; Aw[4 * N + env] = target_spd;
-        Aw[5 * N + env] = target_angle; Aw[6 * N + env] = last_len; Aw[7 * N + env] = total_spd; Aw[8 * N + env] = max_spd;
-        Aw[9 * N + env] = push_count; Aw[10 * N + env] = pf[0]; Aw[11 * N + env] = pf[1]; Aw[12 * N + env] = pf[2];
-        Aw[14 * N + env] = push_draws; Aw[15 * N + env] = cmd_draws;
+        Aw[LLQ_AUX_COUNTER * N + env] = counter; Aw[LLQ_AUX_CMD_FREQ * N + env] = cmd_freq; Aw[LLQ_AUX_TARGET_X * N + env] = tgx;
+        Aw[LLQ_AUX_TARGET_Y * N + env] = tgy; Aw[LLQ_AUX_TARGET_SPD * N + env] = target_spd;
+        Aw[LLQ_AUX_TARGET_ANGLE * N + env] = target_angle; Aw[LLQ_AUX_LAST_POS_DIFF_LEN * N + env] = last_len;
+        Aw[LLQ_AUX_TOTAL_SPD * N + env] = total_spd; Aw[LLQ_AUX_MAX_SPD * N + env] = max_spd;
+        Aw[LLQ_AUX_PUSH_COUNT * N + env] = push_count; Aw[LLQ_AUX_PUSH_F * N + env] = pf[0]; Aw[(LLQ_AUX_PUSH_F + 1) * N + env] = pf[1]; Aw[(LLQ_AUX_PUSH_F + 2) * N + env] = pf[2];
+        Aw[LLQ_AUX_PUSH_DRAWS * N + env] = push_draws; Aw[LLQ_AUX_CMD_DRAWS * N + env] = cmd_draws;
       }
     }
   }
@@ -803,11 +770,11 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
   const long long pair_gid = gid0 + (env & ~1);
   if (ENV != 0) {
     const double* A = E.aux;
-    push_count = (int)A[9 * N + env];
-    pf[0] = (float)A[10 * N + env]; pf[1] = (float)A[11 * N + env]; pf[2] = (float)A[12 * N + env];
-    mu_env = P.mu_ground * (float)A[13 * N + env]; push_draws = (int)A[14 * N + env];
+    push_count = (int)A[LLQ_AUX_PUSH_COUNT * N + env];
+    pf[0] = (float)A[LLQ_AUX_PUSH_F * N + env]; pf[1] = (float)A[(LLQ_AUX_PUSH_F + 1) * N + env]; pf[2] = (float)A[(LLQ_AUX_PUSH_F + 2) * N + env];
+    mu_env = P.mu_ground * (float)A[LLQ_AUX_FOOT_FRICTION * N + env]; push_draws = (int)A[LLQ_AUX_PUSH_DRAWS * N + env];
     epi = E.episode[env] - 1;                             // streams of the running episode (the reset advanced the counter)
-    if (ENV == 2) { PS.flag_x = A[2 * N + env]; PS.flag_y = A[3 * N + env]; }
+    if (ENV == 2) { PS.flag_x = A[LLQ_AUX_FLAG_X * N + env]; PS.flag_y = A[LLQ_AUX_FLAG_Y * N + env]; }
   }
   // ---- EPMC corridor: the boxes the robot can reach during this step -> shared memory (<= kMaxCand per env)
   int n_cand = 0;
@@ -849,7 +816,8 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
       if (push_count > 0) {
         if (push_count % P.push_interval == 0) { push_draws += 1; push_count = 0; }
         if (push_count < P.push_duration) {
-          push_force_of_draw(P, seed, pair_gid, epi, push_draws - 1 + robot, pf);
+          int d = push_draws - 1 + robot;
+          epmc_randomize_push(P, seed, pair_gid, epi, d, pf);
           push_draws += 2;
           push_on = true;
         }

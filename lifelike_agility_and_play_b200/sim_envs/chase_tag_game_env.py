@@ -96,17 +96,17 @@ class ChaseTagGameEnv:
     @property
     def with_flag(self):
         aux = self._engine.get(capi.F_AUX)
-        return [bool(aux[0, 1]), bool(aux[1, 1])]
+        return [bool(aux[0, capi.AUX_WITH_FLAG]), bool(aux[1, capi.AUX_WITH_FLAG])]
 
     @property
     def oppo_visible(self):
         aux = self._engine.get(capi.F_AUX)
-        return np.array([bool(aux[0, 5]), bool(aux[1, 5])])
+        return np.array([bool(aux[0, capi.AUX_OPPO_VISIBLE]), bool(aux[1, capi.AUX_OPPO_VISIBLE])])
 
     @property
     def target_pos(self):
         aux = self._engine.get(capi.F_AUX)
-        return [float(aux[0, 2]), float(aux[0, 3]), 0.25]
+        return [float(aux[0, capi.AUX_FLAG_X]), float(aux[0, capi.AUX_FLAG_Y]), 0.25]
 
     def reset(self, **kwargs):
         obs = self._engine.reset()                                                           # CTG:261-304
@@ -116,8 +116,9 @@ class ChaseTagGameEnv:
         a = np.stack([np.asarray(x['A_LLC'], dtype=np.float32).reshape(12) for x in rl_actions])      # CTG:379
         obs, reward, done = self._engine.step(a)
         aux = self._engine.get(capi.F_AUX)
-        info = {'avg_spd0': float(aux[0, 7] / aux[0, 0]), 'avg_spd1': float(aux[1, 7] / aux[1, 0]),  # CTG:402-407
-                'max_spd0': float(aux[0, 8]), 'max_spd1': float(aux[1, 8])}
+        spd = aux[:, capi.AUX_TOTAL_SPD] / aux[:, capi.AUX_COUNTER]
+        info = {'avg_spd0': float(spd[0]), 'avg_spd1': float(spd[1]),                                  # CTG:402-407
+                'max_spd0': float(aux[0, capi.AUX_MAX_SPD]), 'max_spd1': float(aux[1, capi.AUX_MAX_SPD])}
         return [self._split(obs[0]), self._split(obs[1])], [float(reward[0]), float(reward[1])], bool(done[0]), info
 
     def close(self):

@@ -108,14 +108,14 @@ class PlayGroundEnv:
     def reset(self, **kwargs):
         self.episodic_reward = OrderedDict({'reward_vel': 0.0, 'reward_rotation': 0.0, 'reward_dist': 0.0, 'reward_avg_spd': 0.0})   # PGE:228
         obs = self._split(self._engine.reset()[0])                                           # PGE:196-249
-        self._last_len = float(self._engine.get(capi.F_AUX)[0][6])
+        self._last_len = float(self._engine.get(capi.F_AUX)[0][capi.AUX_LAST_POS_DIFF_LEN])
         return obs
 
     def _episodic_terms(self, aux, reward, done):
         """The per-term sums the reference reports in `info` on termination (PGE:354-357, 498-501, 527-538), restated on the host from
         the step's post-state: the kernel returns the summed reward only."""
         st = self._engine.get(capi.F_STATE)[0].astype(np.float64)
-        d = np.array([aux[2] - st[0], aux[3] - st[1]])
+        d = np.array([aux[capi.AUX_TARGET_X] - st[0], aux[capi.AUX_TARGET_Y] - st[1]])
         plen = float(np.linalg.norm(d))
         u = d / plen
         x, y, z, w = st[3:7] / np.linalg.norm(st[3:7])
@@ -124,9 +124,9 @@ class PlayGroundEnv:
         if self.reward_type == 'joystick':
             spd = abs(st[7] * u[0] + st[8] * u[1])
             self.episodic_reward['reward_rotation'] += reward_rotation / float(self._max_steps)
-            self.episodic_reward['reward_vel'] += float(np.exp(-abs(spd - aux[4]))) / float(self._max_steps)
+            self.episodic_reward['reward_vel'] += float(np.exp(-abs(spd - aux[capi.AUX_TARGET_SPD]))) / float(self._max_steps)
         else:
-            init_len = float(aux[17])
+            init_len = float(aux[capi.AUX_INIT_POS_DIFF_LEN])
             scaled_rot = reward_rotation / float(self._max_steps) * 0.1
             scaled_dist = -((plen - self._last_len) / init_len) * 0.1
             self._last_len = plen
@@ -142,8 +142,8 @@ class PlayGroundEnv:
         aux = self._engine.get(capi.F_AUX)[0]
         self._episodic_terms(aux, reward[0], bool(done[0]))
         if done[0]:                                                                           # PGE:345-357
-            info['ave_spd'] = float(aux[7] / aux[0])
-            info['max_spd'] = float(aux[8])
+            info['ave_spd'] = float(aux[capi.AUX_TOTAL_SPD] / aux[capi.AUX_COUNTER])
+            info['max_spd'] = float(aux[capi.AUX_MAX_SPD])
             for key in ('reward_vel', 'reward_rotation', 'reward_dist', 'reward_avg_spd'):
                 info[key] = self.episodic_reward[key]
         return self._split(obs[0]), float(reward[0]), bool(done[0]), info

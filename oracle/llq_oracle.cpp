@@ -1846,16 +1846,19 @@ int llq_get_field(llq_handle h, int field, void* dst) {
       case LLQ_F_OBS: std::memcpy((float*)dst + (size_t)i * h->obs_dim(), e.obs, sizeof(float) * h->obs_dim()); break;
       case LLQ_F_AUX: {
         double* a = (double*)dst + (size_t)i * LLQ_AUX_DIM;
+        a[LLQ_AUX_COUNTER] = e.counter; a[LLQ_AUX_TOTAL_SPD] = e.total_spd; a[LLQ_AUX_MAX_SPD] = e.max_spd;
+        a[LLQ_AUX_PUSH_COUNT] = e.push_count;
+        for (int t = 0; t < 3; t++) a[LLQ_AUX_PUSH_F + t] = e.push_f[t];
+        a[LLQ_AUX_FOOT_FRICTION] = e.foot_mu; a[LLQ_AUX_PUSH_DRAWS] = e.push_draws; a[LLQ_AUX_YAW_ACCUM_DEG] = e.yaw_accum_deg;
         if (h->cfg.env_kind == LLQ_ENV_SEPMC) {
-          a[0] = e.counter; a[1] = e.with_flag; a[2] = e.flag_x; a[3] = e.flag_y; a[4] = e.fix_spd; a[5] = e.visible; a[6] = e.switch_flag;
-          a[7] = e.total_spd; a[8] = e.max_spd; a[9] = e.push_count; a[10] = e.push_f[0]; a[11] = e.push_f[1]; a[12] = e.push_f[2];
-          a[13] = e.foot_mu; a[14] = e.push_draws; a[15] = e.flag_draws; a[16] = e.yaw_accum_deg; a[17] = e.touch;
-          break;
+          a[LLQ_AUX_WITH_FLAG] = e.with_flag; a[LLQ_AUX_FLAG_X] = e.flag_x; a[LLQ_AUX_FLAG_Y] = e.flag_y; a[LLQ_AUX_CONTROL_SPD] = e.fix_spd;
+          a[LLQ_AUX_OPPO_VISIBLE] = e.visible; a[LLQ_AUX_SWITCH_FLAG] = e.switch_flag; a[LLQ_AUX_FLAG_DRAWS] = e.flag_draws;
+          a[LLQ_AUX_FLAG_TOUCH] = e.touch;
+        } else {
+          a[LLQ_AUX_CMD_FREQ] = e.cmd_freq; a[LLQ_AUX_TARGET_X] = e.tgt_x; a[LLQ_AUX_TARGET_Y] = e.tgt_y; a[LLQ_AUX_TARGET_SPD] = e.target_spd;
+          a[LLQ_AUX_TARGET_ANGLE] = e.target_angle; a[LLQ_AUX_LAST_POS_DIFF_LEN] = e.last_pos_diff_len; a[LLQ_AUX_CMD_DRAWS] = e.cmd_draws;
+          a[LLQ_AUX_INIT_POS_DIFF_LEN] = e.init_pos_diff_len;
         }
-        a[0] = e.counter; a[1] = e.cmd_freq; a[2] = e.tgt_x; a[3] = e.tgt_y; a[4] = e.target_spd; a[5] = e.target_angle;
-        a[6] = e.last_pos_diff_len; a[7] = e.total_spd; a[8] = e.max_spd; a[9] = e.push_count; a[10] = e.push_f[0];
-        a[11] = e.push_f[1]; a[12] = e.push_f[2]; a[13] = e.foot_mu; a[14] = e.push_draws; a[15] = e.cmd_draws;
-        a[16] = e.yaw_accum_deg; a[17] = e.init_pos_diff_len;
         break;
       }
       case LLQ_F_EPISODE_ID: ((int64_t*)dst)[i] = e.episode; break;
@@ -1903,17 +1906,19 @@ int llq_set_field(llq_handle h, int field, const void* src) {
       case LLQ_F_OB_ID: e.ob_id = ((const int32_t*)src)[i]; break;
       case LLQ_F_AUX: {
         const double* a = (const double*)src + (size_t)i * LLQ_AUX_DIM;
+        e.counter = (int)a[LLQ_AUX_COUNTER]; e.total_spd = a[LLQ_AUX_TOTAL_SPD]; e.max_spd = a[LLQ_AUX_MAX_SPD];
+        e.push_count = (int)a[LLQ_AUX_PUSH_COUNT];
+        for (int t = 0; t < 3; t++) e.push_f[t] = a[LLQ_AUX_PUSH_F + t];
+        e.foot_mu = a[LLQ_AUX_FOOT_FRICTION]; e.push_draws = (int)a[LLQ_AUX_PUSH_DRAWS]; e.yaw_accum_deg = a[LLQ_AUX_YAW_ACCUM_DEG];
         if (h->cfg.env_kind == LLQ_ENV_SEPMC) {
-          e.counter = (int)a[0]; e.with_flag = (int)a[1]; e.flag_x = a[2]; e.flag_y = a[3]; e.fix_spd = a[4]; e.visible = (int)a[5];
-          e.switch_flag = (int)a[6]; e.total_spd = a[7]; e.max_spd = a[8]; e.push_count = (int)a[9]; e.push_f[0] = a[10]; e.push_f[1] = a[11];
-          e.push_f[2] = a[12]; e.foot_mu = a[13]; e.push_draws = (int)a[14]; e.flag_draws = (int)a[15]; e.yaw_accum_deg = a[16];
-          e.touch = (int)a[17];
+          e.with_flag = (int)a[LLQ_AUX_WITH_FLAG]; e.flag_x = a[LLQ_AUX_FLAG_X]; e.flag_y = a[LLQ_AUX_FLAG_Y]; e.fix_spd = a[LLQ_AUX_CONTROL_SPD];
+          e.visible = (int)a[LLQ_AUX_OPPO_VISIBLE]; e.switch_flag = (int)a[LLQ_AUX_SWITCH_FLAG]; e.flag_draws = (int)a[LLQ_AUX_FLAG_DRAWS];
+          e.touch = (int)a[LLQ_AUX_FLAG_TOUCH];
           break;
         }
-        e.counter = (int)a[0]; e.cmd_freq = (int)a[1]; e.tgt_x = a[2]; e.tgt_y = a[3]; e.target_spd = a[4]; e.target_angle = a[5];
-        e.last_pos_diff_len = a[6]; e.total_spd = a[7]; e.max_spd = a[8]; e.push_count = (int)a[9]; e.push_f[0] = a[10];
-        e.push_f[1] = a[11]; e.push_f[2] = a[12]; e.foot_mu = a[13]; e.push_draws = (int)a[14]; e.cmd_draws = (int)a[15];
-        e.yaw_accum_deg = a[16]; e.init_pos_diff_len = a[17];
+        e.cmd_freq = (int)a[LLQ_AUX_CMD_FREQ]; e.tgt_x = a[LLQ_AUX_TARGET_X]; e.tgt_y = a[LLQ_AUX_TARGET_Y]; e.target_spd = a[LLQ_AUX_TARGET_SPD];
+        e.target_angle = a[LLQ_AUX_TARGET_ANGLE]; e.last_pos_diff_len = a[LLQ_AUX_LAST_POS_DIFF_LEN]; e.cmd_draws = (int)a[LLQ_AUX_CMD_DRAWS];
+        e.init_pos_diff_len = a[LLQ_AUX_INIT_POS_DIFF_LEN];
         if (e.cmd_freq <= 0) return fail(LLQ_EINVAL, "cmd_vary_freq must be positive");
         break;
       }

@@ -25,6 +25,14 @@ def test_both_libraries_export_every_declared_symbol(built):
             assert hasattr(lib, n), "%s does not export %s" % (path, n)
 
 
+def test_field_ids_and_aux_slots_match_header():
+    txt = open(os.path.join(ROOT, "include", "llq.h")).read()
+    defs = re.findall(r"^#define LLQ_((?:F|AUX)_\w+)\s+(\d+)", txt, re.M)
+    assert len(defs) >= 16 + 25
+    for name, value in defs:
+        assert getattr(capi, name) == int(value), name
+
+
 def test_config_struct_matches_header(built, oracle_lib):
     cfg = oracle_lib.default_config()
     assert cfg.struct_size == ctypes.sizeof(capi.LlqConfig)

@@ -19,8 +19,9 @@ SEPMC_CFG = dict(env_kind=2, kp=50.0, kd=0.5, max_tau=16.0, ground_friction=1.0,
 SEG = dict(prop=(0, 99), prop_a=(99, 135), percept_2d=(135, 460), percept_1d=(460, 588), percept_front=(588, 913), percept_vec=(913, 918),
            oppo_info=(918, 933), oppo_info_cheat=(933, 948), flag_info=(948, 955), flag_info_cheat=(955, 962), with_flag=(962, 964),
            control_spd=(964, 965))
-EXACT_AUX = [0, 1, 5, 6, 9, 14, 15]         # counter, with_flag, visible, switch, push count, push draws, flag draws
-CONT_AUX = [2, 3, 4, 7, 8, 13]              # flag xy, speed command, speed stats, friction
+EXACT_AUX = [capi.AUX_COUNTER, capi.AUX_WITH_FLAG, capi.AUX_OPPO_VISIBLE, capi.AUX_SWITCH_FLAG, capi.AUX_PUSH_COUNT, capi.AUX_PUSH_DRAWS,
+             capi.AUX_FLAG_DRAWS]         # counter, with_flag, visible, switch, push count, push draws, flag draws
+CONT_AUX = [capi.AUX_FLAG_X, capi.AUX_FLAG_Y, capi.AUX_CONTROL_SPD, capi.AUX_TOTAL_SPD, capi.AUX_MAX_SPD, capi.AUX_FOOT_FRICTION]              # flag xy, speed command, speed stats, friction
 
 
 @pytest.fixture(scope="module")

@@ -10,6 +10,7 @@ from test_golden_epmc import EPMC_CFG, GOLD
 from test_parity_gpu import MU_A, SIGMA_A, TOL, blockrel
 
 pytestmark = pytest.mark.gpu
+CONT = [capi.AUX_TARGET_X, capi.AUX_TARGET_Y, capi.AUX_TARGET_SPD, capi.AUX_FOOT_FRICTION, capi.AUX_INIT_POS_DIFF_LEN]   # target, speed command, friction, initial distance
 
 
 def _pair(n, blob, oracle_lib, seed, **over):
@@ -166,7 +167,7 @@ def _crowd_terrain(cpu, rng, n):
         elif kind == 2:     # feet at an obstacle's front edge
             st[i, 0] = b[0] - b[3] - rng.uniform(0.15, 0.3); st[i, 1] = rng.uniform(-0.2, 0.2)
         else:               # next to the target
-            st[i, 0] = aux[i, 2] - rng.uniform(0.2, 0.8); st[i, 1] = rng.uniform(-0.2, 0.2); st[i, 2] = 0.35
+            st[i, 0] = aux[i, capi.AUX_TARGET_X] - rng.uniform(0.2, 0.8); st[i, 1] = rng.uniform(-0.2, 0.2); st[i, 2] = 0.35
     cpu.set(capi.F_STATE, st)
 
 
@@ -241,7 +242,7 @@ def test_cuda_replays_reference_epmc_terrain_golden(element, built, blob):
             assert bool(d[0]) == bool(g["done"][step]), ("done", step)
             aux = eng.get(capi.F_AUX)[0]
             assert np.array_equal(aux[T_EXACT], g["aux"][step][T_EXACT]), ("counters", step)
-            assert np.allclose(aux[[2, 3, 4, 13, 17]], g["aux"][step][[2, 3, 4, 13, 17]], rtol=1e-5, atol=1e-6)
+            assert np.allclose(aux[CONT], g["aux"][step][CONT], rtol=1e-5, atol=1e-6)
             step += 1; t += 1
     assert step == len(g["episode"])
     print("CUDA vs reference EPMC element %d golden (state teacher-forced): %d of %d steps deviate by more than 5e-3 (worst %.1e)" % (

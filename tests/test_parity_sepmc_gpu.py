@@ -10,6 +10,7 @@ from test_golden_sepmc import CONT_AUX, EXACT_AUX, GOLD, SEG, SEPMC_CFG, align, 
 from test_parity_gpu import MU_A, SIGMA_A, TOL, blockrel
 
 pytestmark = pytest.mark.gpu
+FLAG_SPD_MU = [capi.AUX_FLAG_X, capi.AUX_FLAG_Y, capi.AUX_CONTROL_SPD, capi.AUX_FOOT_FRICTION]
 FIELDS = (capi.F_STATE, capi.F_WARMSTART, capi.F_OBS, capi.F_TIME, capi.F_AUX, capi.F_EPISODE_ID, capi.F_REWARD_SUM)
 
 
@@ -36,7 +37,7 @@ def test_sepmc_reset_parity(built, blob, oracle_lib):
         og, oc = gpu.reset(), cpu.reset()
         ag, ac = gpu.get(capi.F_AUX), cpu.get(capi.F_AUX)
         assert np.array_equal(ag[:, EXACT_AUX], ac[:, EXACT_AUX])
-        assert np.allclose(ag[:, CONT_AUX + [16]], ac[:, CONT_AUX + [16]], rtol=1e-6, atol=1e-6)
+        assert np.allclose(ag[:, CONT_AUX + [capi.AUX_YAW_ACCUM_DEG]], ac[:, CONT_AUX + [capi.AUX_YAW_ACCUM_DEG]], rtol=1e-6, atol=1e-6)
         assert seg_err(og, oc).max() < TOL
         assert blockrel(gpu.get(capi.F_STATE), cpu.get(capi.F_STATE)).max() < TOL
     gpu.close(); cpu.close()
@@ -49,14 +50,14 @@ def _crowd(cpu, rng, n):
         kind = rng.integers(0, 4)
         r = 2 * p + rng.integers(0, 2)
         if kind == 0:       # onto the flag
-            st[r, 0:2] = aux[r, 2:4] + rng.uniform(-0.25, 0.25, 2)
+            st[r, 0:2] = aux[r, [capi.AUX_FLAG_X, capi.AUX_FLAG_Y]] + rng.uniform(-0.25, 0.25, 2)
         elif kind == 1:     # onto the partner
             st[r, 0:2] = st[r ^ 1, 0:2] + rng.uniform(-0.35, 0.35, 2)
         elif kind == 2:     # into a wall
             ax = rng.integers(0, 2)
             st[r, ax] = rng.choice([-1.0, 1.0]) * rng.uniform(2.2, 2.4)
         else:               # flag right in front of the head
-            st[r, 0:2] = aux[r, 2:4] - 0.35 * np.array([1 - 2 * (st[r, 4] ** 2 + st[r, 5] ** 2), 2 * (st[r, 3] * st[r, 4] + st[r, 5] * st[r, 6])])
+            st[r, 0:2] = aux[r, [capi.AUX_FLAG_X, capi.AUX_FLAG_Y]] - 0.35 * np.array([1 - 2 * (st[r, 4] ** 2 + st[r, 5] ** 2), 2 * (st[r, 3] * st[r, 4] + st[r, 5] * st[r, 6])])
     cpu.set(capi.F_STATE, st)
 
 
@@ -73,7 +74,7 @@ def _sweep(gpu, cpu, n, steps, rng, crowd_every=3):
         ag, ac = gpu.get(capi.F_AUX), cpu.get(capi.F_AUX)
         m = cpu.get(capi.F_DECISION_MARGIN)
         # discrete outcomes (touch / tag / visibility / counters) must agree except right at a geometric threshold
-        disc = np.any(ag[:, EXACT_AUX + [17]] != ac[:, EXACT_AUX + [17]], axis=1) | (dg != dc) | (np.abs(rg - rc) > 1e-6)
+        disc = np.any(ag[:, EXACT_AUX + [capi.AUX_FLAG_TOUCH]] != ac[:, EXACT_AUX + [capi.AUX_FLAG_TOUCH]], axis=1) | (dg != dc) | (np.abs(rg - rc) > 1e-6)
         e = np.maximum(seg_err(og, oc), blockrel(gpu.get(capi.F_STATE), cpu.get(capi.F_STATE)))
         assert np.allclose(ag[~disc][:, [2, 3, 4, 13]], ac[~disc][:, [2, 3, 4, 13]], rtol=1e-6, atol=1e-6), "flag position / speed command / friction"
         ok = ~disc & (e < TOL)
@@ -153,7 +154,7 @@ def test_cuda_replays_reference_sepmc_golden(built, blob):
             assert bool(d[0]) == bool(d[1]) == bool(g["done"][step]), ("done", step)
             aux = eng.get(capi.F_AUX)
             assert np.array_equal(aux[:, EXACT_AUX], g["aux"][step][:, EXACT_AUX]), ("discrete", step, aux[:, EXACT_AUX], g["aux"][step][:, EXACT_AUX])
-            assert np.allclose(aux[:, [2, 3, 4, 13]], g["aux"][step][:, [2, 3, 4, 13]], rtol=1e-5, atol=1e-6), ("flag / speed / friction", step)
+            assert np.allclose(aux[:, FLAG_SPD_MU], g["aux"][step][:, FLAG_SPD_MU], rtol=1e-5, atol=1e-6), ("flag / speed / friction", step)
             step += 1; t += 1
     assert step == len(g["episode"])
     print("CUDA vs reference SEPMC golden (state teacher-forced): %d of %d steps deviate by more than 5e-3 %s; every reward / done / counter equal" % (

@@ -62,7 +62,7 @@ def designed(kind, element, oracle_lib):
             e = make(oracle_lib, kind, element, n)
             aux = e.get(capi.F_AUX)
             e.close()
-            aux[:, 2] = np.repeat(flags[:, 0], 2); aux[:, 3] = np.repeat(flags[:, 1], 2)
+            aux[:, capi.AUX_FLAG_X] = np.repeat(flags[:, 0], 2); aux[:, capi.AUX_FLAG_Y] = np.repeat(flags[:, 1], 2)
             _BATCHES[key] = (n, states, aux, cats, vis)
         elif element == 0:
             states, cats = pc.flat_batch(rng, N_FLAT)
@@ -113,7 +113,7 @@ def reference_rows(kind, st, aux, boxes, nbox):
     if kind == "sepmc":
         for p in range(n // 2):
             a, b = st[2 * p].astype(np.float64), st[2 * p + 1].astype(np.float64)
-            vis = pc.visible(a, b, pc.arena_boxes(aux[2 * p, 2], aux[2 * p, 3]))
+            vis = pc.visible(a, b, pc.arena_boxes(aux[2 * p, capi.AUX_FLAG_X], aux[2 * p, capi.AUX_FLAG_Y]))
             for i, (s, o) in enumerate(((a, b), (b, a))):
                 v, s_ = pc.sepmc_row(s, o, aux[2 * p + i], aux[2 * p + 1 - i], vis[i])
                 V.append(v); S.append(s_)
@@ -129,7 +129,7 @@ def post_pose_decisive(kind, st, aux, boxes, nbox):
     ok = []
     for i in range(len(st)):
         s = st[i].astype(np.float64)
-        bx = pc.arena_boxes(aux[i, 2], aux[i, 3]) if kind == "sepmc" else (pc.corridor_boxes(boxes[i, :nbox[i]]) if nbox[i] > 0 else pc.SLAB)
+        bx = pc.arena_boxes(aux[i, capi.AUX_FLAG_X], aux[i, capi.AUX_FLAG_Y]) if kind == "sepmc" else (pc.corridor_boxes(boxes[i, :nbox[i]]) if nbox[i] > 0 else pc.SLAB)
         ok.append(pc.rays_decisive(s[0:3], pc.rot(s[3:7]), bx))
     return np.array(ok)
 
@@ -145,8 +145,8 @@ def test_the_oracle_matches_the_caster_ray_by_ray(kind, element, oracle_lib):
     n, designed_states, _, _, vis = designed(kind, element, oracle_lib)
     assert_pose_kept(st, designed_states)
     if kind == "sepmc":
-        assert not aux[:, 6].any(), "a flag switch moved the flag during the step"
-        assert np.array_equal(aux[:, 5] != 0, vis), "oppo_visible"
+        assert not aux[:, capi.AUX_SWITCH_FLAG].any(), "a flag switch moved the flag during the step"
+        assert np.array_equal(aux[:, capi.AUX_OPPO_VISIBLE] != 0, vis), "oppo_visible"
     ref, S = reference_rows(kind, st, aux, boxes, nbox)
     got = obs[:, 135:].astype(np.float64)
     err = np.abs(got - ref)
@@ -168,7 +168,7 @@ def test_the_designed_batches_reach_every_category(kind, element, oracle_lib):
     # every env reaches what its category is named for
     if kind == "sepmc":
         assert vis.any() and not vis.all(), "pairs on both sides of oppo_visible"
-        missed = [(p, cats[p]) for p in range(n // 2) if not pc.reaches("sepmc", cats[p], states[2 * p], pc.arena_boxes(aux[2 * p, 2], aux[2 * p, 3]))]
+        missed = [(p, cats[p]) for p in range(n // 2) if not pc.reaches("sepmc", cats[p], states[2 * p], pc.arena_boxes(aux[2 * p, capi.AUX_FLAG_X], aux[2 * p, capi.AUX_FLAG_Y]))]
     elif element == 0:
         missed = [(i, cats[i]) for i in range(n) if not pc.reaches("flat", cats[i], states[i], pc.SLAB)]
     else:

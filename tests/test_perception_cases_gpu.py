@@ -38,9 +38,9 @@ def test_cuda_perception_matches_the_caster_ray_by_ray(kind, element, built, ora
     assert_pose_kept(st, states, qtol=2.5e-7)        # the kernel turns the quaternion into the inertial frame and back in fp32
     assert post_pose_decisive(kind, st, aux, boxes, nbox).all()
     if kind == "sepmc":
-        assert not aux[:, 6].any(), "a flag switch moved the flag during the step"
+        assert not aux[:, capi.AUX_SWITCH_FLAG].any(), "a flag switch moved the flag during the step"
         # the flag blocks or clears every visibility segment by >= 1 cm: the flags are equal, and equal to the builder's
-        assert np.array_equal(aux[:, 5], aux_cpu[:, 5]) and np.array_equal(aux[:, 5] != 0, vis), (aux[:, 5], aux_cpu[:, 5], vis)
+        assert np.array_equal(aux[:, capi.AUX_OPPO_VISIBLE], aux_cpu[:, capi.AUX_OPPO_VISIBLE]) and np.array_equal(aux[:, capi.AUX_OPPO_VISIBLE] != 0, vis), (aux[:, capi.AUX_OPPO_VISIBLE], aux_cpu[:, capi.AUX_OPPO_VISIBLE], vis)
     ref, S = reference_rows(kind, st, aux, boxes, nbox)
     got = obs[:, 135:].astype(np.float64)
     err = np.abs(got - ref)

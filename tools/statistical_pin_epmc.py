@@ -110,8 +110,8 @@ def main():
                 x, y, z, w = st[i, 3:7] / np.linalg.norm(st[i, 3:7])
                 r22 = 1 - 2 * (x * x + y * y)
                 left_z = 2 * (x * z + y * w) * 2 * (x * y + z * w) - 2 * (y * z - x * w) * (1 - 2 * (y * y + z * z))
-                dist = float(np.hypot(aux[i, 2] - st[i, 0], aux[i, 3] - st[i, 1]))
-                cause = "reach" if dist < 0.5 else ("fall" if (r22 < 0.5 or abs(left_z) > 0.7071) else ("timeup" if aux[i, 0] >= cfg["max_steps"] else "other"))
+                dist = float(np.hypot(aux[i, capi.AUX_TARGET_X] - st[i, 0], aux[i, capi.AUX_TARGET_Y] - st[i, 1]))
+                cause = "reach" if dist < 0.5 else ("fall" if (r22 < 0.5 or abs(left_z) > 0.7071) else ("timeup" if aux[i, capi.AUX_COUNTER] >= cfg["max_steps"] else "other"))
                 ep[cause] += 1
                 ep_len.append(int(steps_alive[i])); ep_rew.append(float(rew_sum[i]))
                 ep_progress.append(float(1.0 - dist / max(start_dist[i], 1e-6)))

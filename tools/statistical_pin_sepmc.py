@@ -101,7 +101,7 @@ def main():
                     r22 = 1 - 2 * (x * x + y * y)
                     left_z = 2 * (x * z + y * w) * 2 * (x * y + z * w) - 2 * (y * z - x * w) * (1 - 2 * (y * y + z * z))
                     fell = fell or r22 < 0.5 or abs(left_z) > 0.7071
-                cause = "fall" if fell else ("timeup" if aux[2 * p, 0] >= cfg["max_steps"] else "tag")
+                cause = "fall" if fell else ("timeup" if aux[2 * p, capi.AUX_COUNTER] >= cfg["max_steps"] else "tag")
                 ends[cause] += 1
                 ep_len.append(int(alive[p]))
                 if cause == "tag":
