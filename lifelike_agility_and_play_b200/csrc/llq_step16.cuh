@@ -1377,7 +1377,9 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
       Q4 dq = Q4{sc * ww.x, sc * ww.y, sc * ww.z, chh};
       qp = qnormalize(qmul(dq, qp));
     }
-    bad = bad || !(fabsf(qd[0]) <= P.vmax) || !(fabsf(ww.x) <= P.vmax) || !(fabsf(vw.x) <= P.vmax);
+    // the velocity clamps map NaN to a bound, so a non-finite joint angle is caught on the angle itself: the EPMC reward does not
+    // read the joints, and without this a robot with a NaN joint angle would step on with its NaN state
+    bad = bad || !(fabsf(qd[0]) <= P.vmax) || !(fabsf(ww.x) <= P.vmax) || !(fabsf(vw.x) <= P.vmax) || !isfinite(q[0] + q[1] + q[2]);
     // ---------------- mocap clock (PLE:208-210): sampled with the time *before* the increment
     if (ENV == 0 && sub == P.substeps - 1) {
       frame_id = (int)floor(time / P.frame_dt);
