@@ -20,7 +20,38 @@ namespace llq {
 constexpr int kObsDim = 207, kObsDimEpmc = 916, kObsDimSepmc = 965, kPropDim = 33, kActDim = 12, kStateDim = 37, kAuxDim = 18;
 template <int ENV> struct ObsW { static constexpr int value = (ENV == 1 || ENV == 3) ? kObsDimEpmc : (ENV == 2 ? kObsDimSepmc : kObsDim); };
 constexpr int kMaxBoxes = 36, kMaxCand = 12;   // ENV 3 = EPMC corridor (elements 1-3): static boxes per env, contact candidates per step
+
+// Staging row: kNewObs floats per env in shared memory.  The step tail and the reset kernel fill it, emit_obs_rows turns it into the
+// observation row.  Shared slots first, then the EPMC names, then the SEPMC names of the same offsets.
 constexpr int kNewObs = 120;
+constexpr int kSQ = 0, kSQd = 12;     // prop 33: joint positions 12 | joint velocities 12 | base part 9
+constexpr int kSPropBase = 24;        //   base part: R^T w 3 | R^T v 3 | R[2,:] 3
+constexpr int kSAct = kPropDim;       // action 12
+constexpr int kSFuture = 45;          // PMC: four future targets of 18
+constexpr int kSRot = 45;             // EPMC, SEPMC: R (world <- base inertial, row major) 9
+constexpr int kSPos = 54;             // EPMC, SEPMC: base position 3
+constexpr int kSTarget = 57;          // EPMC: unit direction to the target in base xy 2
+constexpr int kSTargetSpd = 59;       // EPMC: target_spd
+constexpr int kSPosNorm = 60;         // EPMC: |base position|
+constexpr int kSCorrYaw = 61;         // EPMC corridor: yaw
+constexpr int kSMaskGrid = 62, kSMaskFront = 64, kSMaskLidar = 66;   // EPMC corridor: candidate box masks, 64 raw bits in 2 floats each
+constexpr int kSFlag = 57;            // SEPMC: flag xy 2, where it stood during the step
+constexpr int kSYaw = 59;             // SEPMC: yaw
+constexpr int kSVec = 62;             // SEPMC: small vectors 52: percept_vec 5, oppo_info 15, oppo_info_cheat 15, flag_info 7,
+                                      //   flag_info_cheat 7, with_flag 2, control_spd 1
+// Before the SEPMC row is staged, the pair's robots exchange points in world coordinates through it: sepmc_pair_tail's convex points
+// (per leg foot 3 and wheel 3, handle 3 on legs 0 and 1), and the step kernel's contact points of the last sub-step (one record per
+// leg: foot | wheel | hip | two body corners | handle, 3 floats each).
+constexpr int kSCvxFoot = 0, kSCvxWheel = 12, kSCvxHandle = 24;
+constexpr int kSContactRec = 18;
+
+// Observation columns: three props, oldest first | prop_a: two actions of the history, this step's action | from kOFuture: PMC four
+// future targets; EPMC, SEPMC perception (down-ray grid 25 x 13, lidar 128, front rays 25 x 13), then the staged tail (EPMC target,
+// SEPMC small vectors).
+constexpr int kOPropA = 3 * kPropDim, kOFuture = kOPropA + 3 * kActDim;
+constexpr int kOGrid = kOFuture, kOLidar = kOGrid + 25 * 13, kOFront = kOLidar + 128, kOTail = kOFront + 25 * 13;
+// Per-env history carry between steps: prop[33:99] | prop_a[12:36]
+constexpr int kHistProp = 2 * kPropDim, kHistAct = 2 * kActDim, kHist = kHistProp + kHistAct;
 
 struct DampItem { float m; float c[3]; float Ic[6]; };
 struct JointConst {
@@ -93,6 +124,7 @@ LLQ_DI float gsum4(float v) {  // sum over the 4 lanes of an env, result on all 
   return v;
 }
 LLQ_DI V3 ld3(const float* p) { return V3{p[0], p[1], p[2]}; }
+LLQ_DI void st3(float* p, V3 v) { p[0] = v.x; p[1] = v.y; p[2] = v.z; }
 LLQ_DI Sym3 ldsym(const float* p) { return Sym3{p[0], p[1], p[2], p[3], p[4], p[5]}; }
 
 // spatial motion / force vectors (angular, linear) at a link origin, link coordinates
@@ -129,6 +161,34 @@ LLQ_DI V3 foot_in_base(const LegConst& L, float q1, float q2, float q3) {
   p = rot<1>(p, c2, s2) + ld3(L.j[1].r);
   p = rot<0>(p, c1, s1) + ld3(L.j[0].r);
   return p;
+}
+// this lane's foot in world coordinates for the base pose qp (world <- B') at (px, py, pz); `off` receives its offset from (px, py, pz)
+LLQ_DI V3 foot_world(const LegConst& L, Q4 qp, const float (&q)[3], double px, double py, double pz, V3* off = nullptr) {
+  const V3 f = mul(qmat(qp), foot_in_base(L, q[0], q[1], q[2]));
+  if (off) *off = f;
+  return V3{(float)px + f.x, (float)py + f.y, (float)pz + f.z};
+}
+
+// Staging-row writers: this lane's joints; (lane 0) the prop base part; the prop base part, rotation and position of an EPMC or SEPMC
+// row; the EPMC target block
+LLQ_DI void stage_joints(float* snew, int k, const float (&q)[3], const float (&qd)[3]) {
+#pragma unroll
+  for (int t = 0; t < 3; t++) { snew[kSQ + 3 * k + t] = q[t]; snew[kSQd + 3 * k + t] = qd[t]; }
+}
+LLQ_DI void stage_prop_base(float* snew, const M3& R, V3 wl, V3 vl) {
+  st3(snew + kSPropBase, wl); st3(snew + kSPropBase + 3, vl); st3(snew + kSPropBase + 6, V3{R.a20, R.a21, R.a22});
+}
+LLQ_DI void stage_pose(float* snew, const M3& R, V3 wl, V3 vl, V3 pos) {
+  stage_prop_base(snew, R, wl, vl);
+  st3(snew + kSRot, V3{R.a00, R.a01, R.a02}); st3(snew + kSRot + 3, V3{R.a10, R.a11, R.a12}); st3(snew + kSRot + 6, V3{R.a20, R.a21, R.a22});
+  st3(snew + kSPos, pos);
+}
+// the target (tgx, tgy, 0) seen from the base at (px, py, pz) in base xy, normalised; target_spd; |base position|
+LLQ_DI void stage_target(float* snew, const M3& R, double px, double py, double pz, double tgx, double tgy, float target_spd) {
+  const V3 d = tmul(R, V3{(float)(tgx - px), (float)(tgy - py), (float)(0.0 - pz)});
+  const float n2 = sqrtf(d.x * d.x + d.y * d.y);
+  snew[kSTarget] = d.x / n2; snew[kSTarget + 1] = d.y / n2; snew[kSTargetSpd] = target_spd;
+  snew[kSPosNorm] = (float)sqrt(px * px + py * py + pz * pz);
 }
 
 // Robot write-back shared by the step tail and the reset kernel: lane k stores its leg's joints and foot (world), lane 0 the base
@@ -268,8 +328,6 @@ LLQ_DI void leg_points(const ModelConst& M, const LegConst& L, int k, const floa
   foot = rot<0>(f, c1, s1) + hip;
 }
 
-// staging row of SEPMC (kNewObs floats per robot): prop 33 | action 12 | R 9 (45) | pos 3 (54) | flag xy 2 (57) | yaw 1 (59) | pad 2 |
-// small vectors 52 (62): percept_vec 5, oppo_info 15, oppo_info_cheat 15, flag_info 7, flag_info_cheat 7, with_flag 2, control_spd 1
 struct PairState { int with_flag, flag_draws, visible, sw; double flag_x, flag_y; };
 
 // End-of-step pair logic shared by the step and the reset kernels (CTG:495-596, 472-493): visibility, flag switch, the small
@@ -283,13 +341,9 @@ LLQ_DI void sepmc_pair_tail(const ModelConst& M, const LegConst& L, int k, int r
   {
     V3 hip, wheel, foot;
     leg_points(M, L, k, q, hip, wheel, foot);
-    const V3 fw = pos + mul(Rp, foot), ww_ = pos + mul(Rp, wheel);
-    snew[3 * k] = fw.x; snew[3 * k + 1] = fw.y; snew[3 * k + 2] = fw.z;
-    snew[12 + 3 * k] = ww_.x; snew[13 + 3 * k] = ww_.y; snew[14 + 3 * k] = ww_.z;
-    if (k < 2) {
-      const V3 hw = pos + mul(Rp, V3{M.handle[k][0], M.handle[k][1], M.handle[k][2]});
-      snew[24 + 3 * k] = hw.x; snew[25 + 3 * k] = hw.y; snew[26 + 3 * k] = hw.z;
-    }
+    st3(snew + kSCvxFoot + 3 * k, pos + mul(Rp, foot));
+    st3(snew + kSCvxWheel + 3 * k, pos + mul(Rp, wheel));
+    if (k < 2) st3(snew + kSCvxHandle + 3 * k, pos + mul(Rp, V3{M.handle[k][0], M.handle[k][1], M.handle[k][2]}));
   }
   __syncwarp();
   // partner's root state
@@ -304,11 +358,11 @@ LLQ_DI void sepmc_pair_tail(const ModelConst& M, const LegConst& L, int k, int r
   const V3 ra = robot == 0 ? pos : opos, rb = robot == 0 ? opos : pos;
   bool vis = ray_arena(ra, rb - ra, fx, fy) < 0.f;
   {
-    const V3 head = V3{snew[24], snew[25], snew[26]};
-    const V3 tf = V3{spart[3 * k], spart[3 * k + 1], spart[3 * k + 2]}, tw = V3{spart[12 + 3 * k], spart[13 + 3 * k], spart[14 + 3 * k]};
+    const V3 head = ld3(snew + kSCvxHandle);
+    const V3 tf = ld3(spart + kSCvxFoot + 3 * k), tw = ld3(spart + kSCvxWheel + 3 * k);
     bool any = ray_arena(head, tf - head, fx, fy) < 0.f || ray_arena(head, tw - head, fx, fy) < 0.f;
     if (k < 2) {
-      const V3 th = V3{spart[24 + 3 * k], spart[25 + 3 * k], spart[26 + 3 * k]};
+      const V3 th = ld3(spart + kSCvxHandle + 3 * k);
       any = any || ray_arena(head, th - head, fx, fy) < 0.f;
     }
     int a = any ? 1 : 0;
@@ -340,18 +394,13 @@ LLQ_DI void sepmc_pair_tail(const ModelConst& M, const LegConst& L, int k, int r
     S.flag_x = -2.0 + 4.0 * u[0]; S.flag_y = -2.0 + 4.0 * u[1];
   }
   if (k == 0) {
-    const V3 wl = tmul(Rq, ww), vl = tmul(Rq, vw);
-    snew[24] = wl.x; snew[25] = wl.y; snew[26] = wl.z; snew[27] = vl.x; snew[28] = vl.y; snew[29] = vl.z;
-    snew[30] = Rq.a20; snew[31] = Rq.a21; snew[32] = Rq.a22;
-    snew[45] = Rq.a00; snew[46] = Rq.a01; snew[47] = Rq.a02; snew[48] = Rq.a10; snew[49] = Rq.a11; snew[50] = Rq.a12;
-    snew[51] = Rq.a20; snew[52] = Rq.a21; snew[53] = Rq.a22;
-    snew[54] = pos.x; snew[55] = pos.y; snew[56] = pos.z;
-    snew[57] = (float)ffx; snew[58] = (float)ffy;                       // the flag where it stood during this step
+    stage_pose(snew, Rq, tmul(Rq, ww), tmul(Rq, vw), pos);
+    snew[kSFlag] = (float)ffx; snew[kSFlag + 1] = (float)ffy;
     const float yaw = atan2f(Rq.a10, Rq.a00);
-    snew[59] = yaw;
+    snew[kSYaw] = yaw;
     float sy, cy;
     llq_sincosf(yaw, &sy, &cy);
-    float* v = snew + 62;
+    float* v = snew + kSVec;
     v[0] = pos.x; v[1] = pos.y; v[2] = pos.z; v[3] = cy; v[4] = sy;                          // percept_vec
     const M3 Ro = qmat(qnormalize(oq));
     const float yawo = atan2f(Ro.a10, Ro.a00);
@@ -484,11 +533,14 @@ LLQ_DI void stage_corridor_masks(float* snew, const float* boxes, int nb, int k,
   const unsigned long long mf = box_mask(boxes, nb, k, px, py, pz, 3.35f, false);   // 3 m rays starting up to 0.27 m off the base
   const unsigned long long m1 = box_mask(boxes, nb, k, px, py, pz, 0.f, true);      // horizontal rays at the base height
   if (k == 0) {
-    snew[61] = yaw;
-    snew[62] = __uint_as_float((unsigned)m2); snew[63] = __uint_as_float((unsigned)(m2 >> 32));
-    snew[64] = __uint_as_float((unsigned)mf); snew[65] = __uint_as_float((unsigned)(mf >> 32));
-    snew[66] = __uint_as_float((unsigned)m1); snew[67] = __uint_as_float((unsigned)(m1 >> 32));
+    snew[kSCorrYaw] = yaw;
+    snew[kSMaskGrid] = __uint_as_float((unsigned)m2); snew[kSMaskGrid + 1] = __uint_as_float((unsigned)(m2 >> 32));
+    snew[kSMaskFront] = __uint_as_float((unsigned)mf); snew[kSMaskFront + 1] = __uint_as_float((unsigned)(mf >> 32));
+    snew[kSMaskLidar] = __uint_as_float((unsigned)m1); snew[kSMaskLidar + 1] = __uint_as_float((unsigned)(m1 >> 32));
   }
+}
+LLQ_DI unsigned long long staged_mask(const float* sn, int slot) {
+  return ((unsigned long long)__float_as_uint(sn[slot + 1]) << 32) | __float_as_uint(sn[slot]);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -514,15 +566,9 @@ LLQ_DI ObsCtx build_obs_new(const MocapDev& mc, const StepParams& P, const Model
   }
   qb = qnormalize(qb);
   M3 Rb = qmat(qb);
-  // prop (PLE:247-260): joint_pos | joint_vel | R^T w | R^T v | R[2,:]
-#pragma unroll
-  for (int i = 0; i < 3; i++) { snew[3 * lane4 + i] = q[i]; snew[12 + 3 * lane4 + i] = qd[i]; }
-  if (lane4 == 0) {
-    V3 wl = tmul(Rb, ang), vl = tmul(Rb, lin);
-    snew[24] = wl.x; snew[25] = wl.y; snew[26] = wl.z;
-    snew[27] = vl.x; snew[28] = vl.y; snew[29] = vl.z;
-    snew[30] = Rb.a20; snew[31] = Rb.a21; snew[32] = Rb.a22;
-  }
+  // prop (PLE:247-260)
+  stage_joints(snew, lane4, q, qd);
+  if (lane4 == 0) stage_prop_base(snew, Rb, tmul(Rb, ang), tmul(Rb, lin));
   // future target `lane4` (ML:75-86, PLE:299-317)
   {
     const double tf = lane4 == 0 ? 1. / 30. : (lane4 == 1 ? 1. / 15. : (lane4 == 2 ? 1. / 3. : 1.));
@@ -535,7 +581,7 @@ LLQ_DI ObsCtx build_obs_new(const MocapDev& mc, const StepParams& P, const Model
     V3 rv = q_rotvec(qnormalize(qmul(qconj(qb), qnormalize(kf.q))));
     float angle = norm3(rv);
     float sc = angle / (angle + 1e-8f);
-    float* o18 = snew + 45 + 18 * lane4;
+    float* o18 = snew + kSFuture + 18 * lane4;
     o18[0] = dp.x; o18[1] = dp.y; o18[2] = dp.z;
     o18[3] = sc * rv.x; o18[4] = sc * rv.y; o18[5] = sc * rv.z;
     float ff = (float)ffrac;
@@ -545,14 +591,40 @@ LLQ_DI ObsCtx build_obs_new(const MocapDev& mc, const StepParams& P, const Model
   return o;
 }
 
+// Ray geometry of the perception columns, from the rotation and position an EPMC or SEPMC staging row holds; t = column in the block.
+LLQ_DI M3 staged_rot(const float* sn) {
+  const float* r = sn + kSRot;
+  return M3{r[0], r[1], r[2], r[3], r[4], r[5], r[6], r[7], r[8]};
+}
+// down-ray grid: world xy of grid point t (25 x 13 over 2.4 m x 1.2 m, in the full base frame)
+LLQ_DI float2 grid_point(const float* sn, int t) {
+  const int a = t / 13, b = t - a * 13;
+  const float gx = a == 24 ? 1.2f : -1.2f + (float)a * (2.4f / 24.0f), gy = b == 12 ? 0.6f : -0.6f + (float)b * (1.2f / 12.0f);
+  const M3 R = staged_rot(sn);
+  return make_float2(fmaf(R.a00, gx, fmaf(R.a01, gy, sn[kSPos])), fmaf(R.a10, gx, fmaf(R.a11, gy, sn[kSPos + 1])));
+}
+// lidar: direction (cos, sin, 0) of horizontal ray t of 128 over the full turn from heading yaw
+LLQ_DI V3 lidar_dir(float yaw, int t) {
+  const float ang = yaw + 6.283185307179586f * (float)t * (1.0f / 128.0f);
+  float sa, ca;
+  llq_sincosf(ang, &sa, &ca);
+  return V3{ca, sa, 0.f};
+}
+// front rays: origin of ray t (25 x 13 over base y in [-0.25, 0.25], z in [-0.3, 0.1]) and the ray, 3 m along body +x
+LLQ_DI void front_ray(const float* sn, int t, V3& from, V3& d) {
+  const int a = t / 13, b = t - a * 13;
+  const float y = a == 24 ? 0.25f : -0.25f + (float)a * (0.5f / 24.0f), z = b == 12 ? 0.1f : -0.3f + (float)b * (0.4f / 12.0f);
+  const M3 R = staged_rot(sn);
+  const V3 pos = ld3(sn + kSPos);
+  from = V3{fmaf(R.a01, y, fmaf(R.a02, z, pos.x)), fmaf(R.a11, y, fmaf(R.a12, z, pos.y)), fmaf(R.a21, y, fmaf(R.a22, z, pos.z))};
+  d = V3{3.f * R.a00, 3.f * R.a10, 3.f * R.a20};
+}
+
 // Cooperative, coalesced emission of the 8 observation rows owned by this warp.
 // mode 0 (step):  prop = [old[33:99], new] ; prop_a = [old[12:36], act] ; future = new
 // mode 1 (reset): prop = [new, new, new]  ; prop_a = 0                 ; future = new      (PLE:282-290)
-// `do_row` (bit e of a warp-uniform mask) selects which of the 8 rows are written.
-constexpr int kHist = 90;   // per-env history carry: prop[33:99] (66) | prop_a[12:36] (24)
-
-// staging row (kNewObs floats per env).  PMC: prop 33 | action 12 | future 72.
-// EPMC: prop 33 | action 12 | R (world<-base inertial, row major) 9 | pos 3 | target 3 | |base_pos| 1   (perception is evaluated while the row is written)
+// `do_row` (bit e of a warp-uniform mask) selects which of the 8 rows are written.  EPMC and SEPMC evaluate the perception columns
+// while the row is written.
 template <int ENV, int EPW = 8>   // EPW = envs per warp (8 with 4 lanes per env, 2 with 16)
 LLQ_DI void emit_obs_rows(float* obs, float* obs2, long long obs2_ld, const float* snew_warp, const float* hist_warp, int env0, int n_envs,
                           int mode, unsigned row_mask, const float* boxes_all = nullptr) {
@@ -567,51 +639,41 @@ LLQ_DI void emit_obs_rows(float* obs, float* obs2, long long obs2_ld, const floa
     if (ok) {
       const float* sn = snew_warp + e * kNewObs;
       const float* hs = hist_warp + e * kHist;
-      if (j < 99) {
+      if (j < kOPropA) {
         if (mode == 1) v = sn[j % kPropDim];
-        else v = j < 66 ? hs[j] : sn[j - 66];
-      } else if (j < 135) {
-        int a = j - 99;
+        else v = j < kHistProp ? hs[j] : sn[j - kHistProp];
+      } else if (j < kOFuture) {
+        int a = j - kOPropA;
         if (mode == 1) v = 0.f;
-        else v = a < 24 ? hs[66 + a] : sn[kPropDim + a - 24];
+        else v = a < kHistAct ? hs[kHistProp + a] : sn[kSAct + a - kHistAct];
       } else if (ENV == 0) {
-        v = sn[45 + (j - 135)];
+        v = sn[kSFuture + (j - kOFuture)];
       } else if (ENV == 3) {
         // EPMC corridor perception against the ground slab and the env's candidate boxes (PGE:374-447)
-        const V3 pos = V3{sn[54], sn[55], sn[56]};
+        const V3 pos = ld3(sn + kSPos);
         const float* bxs = boxes_all + (size_t)(env0 + e) * (6 * kMaxBoxes);
-        if (j < 460) {
-          const unsigned long long m = ((unsigned long long)__float_as_uint(sn[63]) << 32) | __float_as_uint(sn[62]);
-          const int t = j - 135, a = t / 13, b = t - a * 13;
-          const float gx = a == 24 ? 1.2f : -1.2f + (float)a * (2.4f / 24.0f), gy = b == 12 ? 0.6f : -0.6f + (float)b * (1.2f / 12.0f);
-          const float x = fmaf(sn[45], gx, fmaf(sn[46], gy, pos.x)), y = fmaf(sn[48], gx, fmaf(sn[49], gy, pos.y));
-          v = fmaxf(down_ray_top(x, y, bxs, m), 0.f);          // hit z of the down ray (0 when it misses everything)
-        } else if (j < 588) {
-          const unsigned long long m = ((unsigned long long)__float_as_uint(sn[67]) << 32) | __float_as_uint(sn[66]);
-          const float ang = sn[61] + 6.283185307179586f * (float)(j - 460) * (1.0f / 128.0f);
-          float sa, ca;
-          llq_sincosf(ang, &sa, &ca);
-          const float f = ray_boxlist(pos, V3{20.f * ca, 20.f * sa, 0.f}, bxs, m);
-          v = f < 0.f ? sn[60] : f * 20.f * sqrtf(ca * ca + sa * sa);
-        } else if (j < 913) {
-          const unsigned long long m = ((unsigned long long)__float_as_uint(sn[65]) << 32) | __float_as_uint(sn[64]);
-          const int t = j - 588, a = t / 13, b = t - a * 13;
-          const float y = a == 24 ? 0.25f : -0.25f + (float)a * (0.5f / 24.0f), z = b == 12 ? 0.1f : -0.3f + (float)b * (0.4f / 12.0f);
-          const V3 from = V3{fmaf(sn[46], y, fmaf(sn[47], z, pos.x)), fmaf(sn[49], y, fmaf(sn[50], z, pos.y)), fmaf(sn[52], y, fmaf(sn[53], z, pos.z))};
-          const V3 d = V3{3.f * sn[45], 3.f * sn[48], 3.f * sn[51]};
-          const float f = ray_boxlist(from, d, bxs, m);
+        if (j < kOLidar) {
+          const float2 g = grid_point(sn, j - kOGrid);
+          v = fmaxf(down_ray_top(g.x, g.y, bxs, staged_mask(sn, kSMaskGrid)), 0.f);   // hit z of the down ray (0 when it misses everything)
+        } else if (j < kOFront) {
+          const V3 u = lidar_dir(sn[kSCorrYaw], j - kOLidar);
+          const float f = ray_boxlist(pos, 20.f * u, bxs, staged_mask(sn, kSMaskLidar));
+          v = f < 0.f ? sn[kSPosNorm] : f * 20.f * sqrtf(u.x * u.x + u.y * u.y);
+        } else if (j < kOTail) {
+          V3 from, d;
+          front_ray(sn, j - kOFront, from, d);
+          const float f = ray_boxlist(from, d, bxs, staged_mask(sn, kSMaskFront));
           v = (f < 0.f ? 1.f : f) * norm3(d);
         } else {
-          v = sn[57 + (j - 913)];
+          v = sn[kSTarget + (j - kOTail)];
         }
       } else if (ENV == 2) {
         // SEPMC perception against ground slab, walls and flag (CTG:598-638, PGE:22-54)
-        const V3 pos = V3{sn[54], sn[55], sn[56]};
-        const float fx = sn[57], fy = sn[58];
-        if (j < 460) {                             // percept_2d: down rays over the 25 x 13 grid in the full base frame, value = hit z
-          const int t = j - 135, a = t / 13, b = t - a * 13;
-          const float gx = a == 24 ? 1.2f : -1.2f + (float)a * (2.4f / 24.0f), gy = b == 12 ? 0.6f : -0.6f + (float)b * (1.2f / 12.0f);
-          const float x = fmaf(sn[45], gx, fmaf(sn[46], gy, pos.x)), y = fmaf(sn[48], gx, fmaf(sn[49], gy, pos.y));
+        const V3 pos = ld3(sn + kSPos);
+        const float fx = sn[kSFlag], fy = sn[kSFlag + 1];
+        if (j < kOLidar) {                         // percept_2d: value = hit z of the down ray
+          const float2 g = grid_point(sn, j - kOGrid);
+          const float x = g.x, y = g.y;
           // a vertical ray sees the highest top among the boxes whose footprint holds (x, y): flag 0.5, walls 2, ground 0
           const bool in_x = fabsf(x) <= 2.5f, in_y = fabsf(y) <= 2.5f;
           const bool wall = (in_x && fabsf(fabsf(y) - 2.5f) <= 0.005f) || (in_y && fabsf(fabsf(x) - 2.5f) <= 0.005f);
@@ -621,40 +683,34 @@ LLQ_DI void emit_obs_rows(float* obs, float* obs2, long long obs2_ld, const floa
             const float f = ray_arena(V3{x, y, 10.f}, V3{0.f, 0.f, -20.f}, fx, fy);
             v = f < 0.f ? 0.f : fmaf(f, -20.f, 10.f);
           }
-        } else if (j < 588) {                      // percept_1d: 128 horizontal rays of 20 m; a miss reports |ray_from|
-          const float ang = sn[59] + 6.283185307179586f * (float)(j - 460) * (1.0f / 128.0f);
-          float sa, ca;
-          llq_sincosf(ang, &sa, &ca);
-          const V3 d = V3{20.f * ca, 20.f * sa, 0.f};
+        } else if (j < kOFront) {                  // percept_1d: rays of 20 m; a miss reports |ray_from|
+          const V3 u = lidar_dir(sn[kSYaw], j - kOLidar);
+          const V3 d = 20.f * u;
           const bool inside = fabsf(pos.x) < 2.49f && fabsf(pos.y) < 2.49f;
           const float f = inside ? ray_arena_inside(pos, d, fx, fy) : ray_arena(pos, d, fx, fy);
-          v = f < 0.f ? norm3(pos) : f * 20.f * sqrtf(ca * ca + sa * sa);
-        } else if (j < 913) {                      // percept_front: 25 x 13 rays of 3 m along body +x; a miss reports 3
-          const int t = j - 588, a = t / 13, b = t - a * 13;
-          const float y = a == 24 ? 0.25f : -0.25f + (float)a * (0.5f / 24.0f), z = b == 12 ? 0.1f : -0.3f + (float)b * (0.4f / 12.0f);
-          const V3 from = V3{fmaf(sn[46], y, fmaf(sn[47], z, pos.x)), fmaf(sn[49], y, fmaf(sn[50], z, pos.y)), fmaf(sn[52], y, fmaf(sn[53], z, pos.z))};
-          const V3 d = V3{3.f * sn[45], 3.f * sn[48], 3.f * sn[51]};
+          v = f < 0.f ? norm3(pos) : f * 20.f * sqrtf(u.x * u.x + u.y * u.y);
+        } else if (j < kOTail) {                   // percept_front: a miss reports 3
+          V3 from, d;
+          front_ray(sn, j - kOFront, from, d);
           const bool inside = fabsf(from.x) < 2.49f && fabsf(from.y) < 2.49f && from.z > 0.f;
           const float f = inside ? ray_arena_inside(from, d, fx, fy) : ray_arena(from, d, fx, fy);
           v = (f < 0.f ? 1.f : f) * norm3(d);
         } else {
-          v = sn[62 + (j - 913)];
+          v = sn[kSVec + (j - kOTail)];
         }
-      } else if (j < 460) {
+      } else if (j < kOLidar) {
         v = 0.f;                                   // percep_2d: every down-ray hits the slab top, hit z = 0 (PGE:431-447)
-      } else if (j < 588) {
-        v = sn[60];                                // percep_1d: horizontal rays miss => |ray_from| (PGE:49-53,388-394)
-      } else if (j < 913) {                        // percep_front (PGE:409-429) against the ground slab
-        int t = j - 588, i = t / 13, jj = t - i * 13;
-        float y = i == 24 ? 0.25f : -0.25f + (float)i * (0.5f / 24.0f);
-        float z = jj == 12 ? 0.1f : -0.3f + (float)jj * (0.4f / 12.0f);
-        float fz = fmaf(sn[52], y, fmaf(sn[53], z, sn[56]));          // from.z = R[2,1] y + R[2,2] z + pos.z
-        float dz = 3.0f * sn[51];                                     // (to - from).z = 3 R[2,0]
-        float len = 3.0f * sqrtf(sn[45] * sn[45] + sn[48] * sn[48] + sn[51] * sn[51]);
-        float tz = fz + dz;
+      } else if (j < kOFront) {
+        v = sn[kSPosNorm];                         // percep_1d: horizontal rays miss => |ray_from| (PGE:49-53,388-394)
+      } else if (j < kOTail) {                     // percep_front (PGE:409-429) against the ground slab
+        V3 from, d;
+        front_ray(sn, j - kOFront, from, d);
+        const M3 R = staged_rot(sn);
+        const float len = 3.0f * sqrtf(R.a00 * R.a00 + R.a10 * R.a10 + R.a20 * R.a20);
+        const float fz = from.z, tz = fz + d.z;
         v = (fz > 0.f && tz < 0.f) ? len * (fz / (fz - tz)) : len;
       } else {
-        v = sn[57 + (j - 913)];
+        v = sn[kSTarget + (j - kOTail)];
       }
       obs[(size_t)(env0 + e) * OW + j] = v;
       if (obs2) obs2[(size_t)(env0 + e) * obs2_ld + j] = v;
@@ -670,7 +726,7 @@ LLQ_DI void prefetch_history(const float* obs, float* hist_warp, int env0, int n
   for (int idx = lane; idx < EPW * kHist; idx += 32) {
     int e = idx / kHist, t = idx - e * kHist;
     int env = env0 + e < n_envs ? env0 + e : n_envs - 1;
-    int j = t < 66 ? 33 + t : 99 + 12 + (t - 66);
+    int j = t < kHistProp ? kPropDim + t : kOPropA + kActDim + (t - kHistProp);
     __pipeline_memcpy_async(hist_warp + idx, obs + (size_t)env * OW + j, 4);
   }
 }
@@ -697,6 +753,24 @@ struct ResetParams {
   double factor;
   int update_table;                           // 1 after a step
 };
+
+// EPMC / SEPMC episode start: init_state turned by yaw_deg about world z; qn in the pybullet inertial-frame convention, qp = world <- B',
+// this lane's joints.  The caller places the base at (px, py, 0.5) and forms the foot where it writes the robot back: computed here,
+// the foot stays live across the corridor generation and the pair tail and costs registers.
+struct StartPose { Q4 qn, qp; float q[3], qd[3]; V3 lin, ang; };
+LLQ_DI StartPose start_pose(const ModelConst& M, int k, double yaw_deg) {
+  StartPose s;
+  double sn, cs;
+  sincos(0.5 * yaw_deg * (3.14159265358979323846 / 180.0), &sn, &cs);
+  const float* I0 = M.init_state;
+  s.qn = qmul(qnormalize(Q4{I0[3], I0[4], I0[5], I0[6]}), Q4{0.f, 0.f, (float)sn, (float)cs});
+#pragma unroll
+  for (int i = 0; i < 3; i++) { s.q[i] = I0[13 + 3 * k + i]; s.qd[i] = I0[25 + 3 * k + i]; }
+  s.lin = V3{I0[7], I0[8], I0[9]}; s.ang = V3{I0[10], I0[11], I0[12]};
+  const Q4 qI = Q4{M.base.qI[0], M.base.qI[1], M.base.qI[2], M.base.qI[3]};
+  s.qp = qmul(qnormalize(s.qn), qconj(qI));
+  return s;
+}
 
 constexpr int kResetBlock = 128;
 template <int ENV>
@@ -781,31 +855,19 @@ __global__ void __launch_bounds__(kResetBlock) pmc_reset_kernel(EnvArrays E, Moc
     // both robots are handed the same mutable init dict => one running yaw for the pair (CTG:209-215)
     const double acc0 = E.aux[LLQ_AUX_YAW_ACCUM_DEG * N + (env & ~1)];
     const double yaw_a = fmod(acc0 + 360.0 * u1[3], 360.0), yaw_b = fmod(yaw_a + 360.0 * u2[0], 360.0);
-    const double yaw_deg = robot == 0 ? yaw_a : yaw_b;
-    double sn, cs;
-    sincos(0.5 * yaw_deg * (3.14159265358979323846 / 180.0), &sn, &cs);
-    const float* I0 = M.init_state;
-    const Q4 qn = qmul(qnormalize(Q4{I0[3], I0[4], I0[5], I0[6]}), Q4{0.f, 0.f, (float)sn, (float)cs});
-    float q[3], qd[3];
-#pragma unroll
-    for (int i = 0; i < 3; i++) { q[i] = I0[13 + 3 * k + i]; qd[i] = I0[25 + 3 * k + i]; }
-    const V3 lin = V3{I0[7], I0[8], I0[9]}, ang = V3{I0[10], I0[11], I0[12]};
-    const Q4 qI = Q4{M.base.qI[0], M.base.qI[1], M.base.qI[2], M.base.qI[3]};
-    const Q4 qp = qmul(qnormalize(qn), qconj(qI));
+    const StartPose S = start_pose(M, k, robot == 0 ? yaw_a : yaw_b);
     PairState PS = {robot == 0 ? wflag : 1 - wflag, 0, 1, 0, -2.0 + 4.0 * u2[1], -2.0 + 4.0 * u2[2]};
     // reset() runs _prepare_drill too (CTG:302): its flag-switch test reads the stale manifolds of the previous episode's last step
     const bool touch_own = E.aux[LLQ_AUX_FLAG_TOUCH * N + env] != 0.0;
-    float* snew = &s_new[threadIdx.x >> 2][0];
-    const float* spart = &s_new[(threadIdx.x >> 2) ^ 1][0];
-    sepmc_pair_tail(M, L, k, robot, snew, spart, px, py, 0.5, qp, qn, lin, ang, q, touch_own, fix_spd, RP.seed, gid, ep, PS);
-#pragma unroll
-    for (int i = 0; i < 3; i++) { snew[3 * k + i] = q[i]; snew[12 + 3 * k + i] = qd[i]; }
+    float* snew = s_new[threadIdx.x >> 2];
+    const float* spart = s_new[(threadIdx.x >> 2) ^ 1];
+    sepmc_pair_tail(M, L, k, robot, snew, spart, px, py, 0.5, S.qp, S.qn, S.lin, S.ang, S.q, touch_own, fix_spd, RP.seed, gid, ep, PS);
+    stage_joints(snew, k, S.q, S.qd);
     int push_draws = 0;
     float pf[3] = {0.f, 0.f, 0.f};
     if (P.push_enabled) push_draws = 1;                              // PR:52-54: draw #0 becomes the current _randomized_force
     if (doit) {
-      V3 f = mul(qmat(qp), foot_in_base(L, q[0], q[1], q[2]));
-      write_robot(E, N, env, k, q, qd, V3{(float)px + f.x, (float)py + f.y, 0.5f + f.z}, px, py, 0.5, qn, lin, ang, 0.0);
+      write_robot(E, N, env, k, S.q, S.qd, foot_world(L, S.qp, S.q, px, py, 0.5), px, py, 0.5, S.qn, S.lin, S.ang, 0.0);
       write_reset(E, N, env, k, ep + 1);
       if (k == 0) {
         double* A = E.aux;
@@ -830,33 +892,21 @@ __global__ void __launch_bounds__(kResetBlock) pmc_reset_kernel(EnvArrays E, Moc
     if (P.push_enabled) epmc_randomize_push(P, RP.seed, gid, ep, push_draws, pf);                          // PR:52-54
     const int cmd_freq = P.cmd_freq_lo + (int)floor(u[2] * (double)(P.cmd_freq_hi - P.cmd_freq_lo));       // PGE:223
     const double yaw_deg = fmod(E.aux[LLQ_AUX_YAW_ACCUM_DEG * N + env] + 360.0 * u[1], 360.0);                                // PGE:181-189 (accumulates)
-    double sn, cs;
-    sincos(0.5 * yaw_deg * (3.14159265358979323846 / 180.0), &sn, &cs);
-    const float* I0 = M.init_state;
-    const Q4 qn = qmul(qnormalize(Q4{I0[3], I0[4], I0[5], I0[6]}), Q4{0.f, 0.f, (float)sn, (float)cs});
-    float q[3], qd[3];
-#pragma unroll
-    for (int i = 0; i < 3; i++) { q[i] = I0[13 + 3 * k + i]; qd[i] = I0[25 + 3 * k + i]; }
-    const V3 lin = V3{I0[7], I0[8], I0[9]}, ang = V3{I0[10], I0[11], I0[12]};
-    float* snew = &s_new[threadIdx.x >> 2][0];
-    const M3 Rq = qmat(qnormalize(qn));
     const float target_spd = (float)E.aux[LLQ_AUX_TARGET_SPD * N + env];            // persists across episodes (PGE:170-172)
     double tgx0 = 8.0;
     int nb0 = 0;
     if (ENV == 3) nb0 = generate_corridor(P, RP.seed, gid, ep, E.boxes + (size_t)env * (6 * kMaxBoxes), doit && k == 0, tgx0);   // PGE:216-219
-#pragma unroll
-    for (int i = 0; i < 3; i++) { snew[3 * k + i] = q[i]; snew[12 + 3 * k + i] = qd[i]; }
+    // the pose after the corridor: generated before it, it is live across generate_corridor (registers).  qn is a local copy and the
+    // foot below keeps the expression with its own qp: read through S or from S.qp, nvcc contracts the quaternion arithmetic differently
+    // and element 0's foot positions change in the last bit.
+    const StartPose S = start_pose(M, k, yaw_deg);
+    const Q4 qn = S.qn;
+    float* snew = s_new[threadIdx.x >> 2];
+    const M3 Rq = qmat(qnormalize(qn));
+    stage_joints(snew, k, S.q, S.qd);
     if (k == 0) {
-      V3 wl = tmul(Rq, ang), vl = tmul(Rq, lin);
-      snew[24] = wl.x; snew[25] = wl.y; snew[26] = wl.z; snew[27] = vl.x; snew[28] = vl.y; snew[29] = vl.z;
-      snew[30] = Rq.a20; snew[31] = Rq.a21; snew[32] = Rq.a22;
-      snew[45] = Rq.a00; snew[46] = Rq.a01; snew[47] = Rq.a02; snew[48] = Rq.a10; snew[49] = Rq.a11; snew[50] = Rq.a12;
-      snew[51] = Rq.a20; snew[52] = Rq.a21; snew[53] = Rq.a22;
-      snew[54] = 0.f; snew[55] = 0.f; snew[56] = 0.5f;
-      V3 d = tmul(Rq, V3{(float)tgx0, 0.f, -0.5f});                 // target - pos (0,0,0.5); element 0: (8,0,0) (BSE:247-248)
-      float n2 = sqrtf(d.x * d.x + d.y * d.y);
-      snew[57] = d.x / n2; snew[58] = d.y / n2; snew[59] = target_spd;
-      snew[60] = 0.5f;
+      stage_pose(snew, Rq, tmul(Rq, S.ang), tmul(Rq, S.lin), V3{0.f, 0.f, 0.5f});
+      stage_target(snew, Rq, 0.0, 0.0, 0.5, tgx0, 0.0, target_spd);                 // element 0: target (8, 0, 0) (BSE:247-248)
     }
     if (ENV == 3) {
       __syncwarp();                                                 // lane 0's boxes are visible to the env's other lanes
@@ -864,8 +914,8 @@ __global__ void __launch_bounds__(kResetBlock) pmc_reset_kernel(EnvArrays E, Moc
     }
     if (doit) {
       const Q4 qI = Q4{M.base.qI[0], M.base.qI[1], M.base.qI[2], M.base.qI[3]};
-      V3 f = mul(qmat(qmul(qnormalize(qn), qconj(qI))), foot_in_base(L, q[0], q[1], q[2]));
-      write_robot(E, N, env, k, q, qd, V3{f.x, f.y, 0.5f + f.z}, 0.0, 0.0, 0.5, qn, lin, ang, 0.0);
+      const V3 f = mul(qmat(qmul(qnormalize(qn), qconj(qI))), foot_in_base(L, S.q[0], S.q[1], S.q[2]));
+      write_robot(E, N, env, k, S.q, S.qd, V3{f.x, f.y, 0.5f + f.z}, 0.0, 0.0, 0.5, qn, S.lin, S.ang, 0.0);
       write_reset(E, N, env, k, ep + 1);
       if (k == 0) {
         double* A = E.aux;
@@ -913,12 +963,11 @@ __global__ void __launch_bounds__(kResetBlock) pmc_reset_kernel(EnvArrays E, Moc
       q[i] = fmaf(fr, n - c, c);
       qd[i] = (n - c) * inv;
     }
-    float* snew = &s_new[threadIdx.x >> 2][0];
-    build_obs_new(mc, P, M, k, clip, frame_id, frac, kb.px, kb.py, kb.pz, kb.q, kb.lin, kb.ang, q, qd, snew);
+    build_obs_new(mc, P, M, k, clip, frame_id, frac, kb.px, kb.py, kb.pz, kb.q, kb.lin, kb.ang, q, qd, s_new[threadIdx.x >> 2]);
     if (doit) {
       const Q4 qI = Q4{M.base.qI[0], M.base.qI[1], M.base.qI[2], M.base.qI[3]};
-      V3 f = mul(qmat(qmul(qnormalize(kb.q), qconj(qI))), foot_in_base(L, q[0], q[1], q[2]));
-      write_robot(E, N, env, k, q, qd, V3{(float)kb.px + f.x, (float)kb.py + f.y, (float)kb.pz + f.z}, kb.px, kb.py, kb.pz, kb.q, kb.lin, kb.ang, t0);
+      const V3 fd = foot_world(L, qmul(qnormalize(kb.q), qconj(qI)), q, kb.px, kb.py, kb.pz);
+      write_robot(E, N, env, k, q, qd, fd, kb.px, kb.py, kb.pz, kb.q, kb.lin, kb.ang, t0);
       write_reset(E, N, env, k, ep);
 #pragma unroll
       for (int i = 0; i < 3; i++) { E.kin[(13 + 3 * k + i) * N + env] = q[i]; E.kin[(25 + 3 * k + i) * N + env] = qd[i]; }
@@ -937,7 +986,7 @@ __global__ void __launch_bounds__(kResetBlock) pmc_reset_kernel(EnvArrays E, Moc
 #pragma unroll
   for (int e = 0; e < 8; e++) if ((wm >> (4 * e)) & 1u) rows |= 1u << e;
   const int warp_env0 = (blockIdx.x * kResetBlock + (threadIdx.x & ~31)) >> 2;
-  emit_obs_rows<ENV>(E.obs, obs2, obs2_ld, &s_new[(threadIdx.x & ~31) >> 2][0], &s_new[0][0], warp_env0, N, 1, rows, E.boxes);
+  emit_obs_rows<ENV>(E.obs, obs2, obs2_ld, s_new[(threadIdx.x & ~31) >> 2], s_new[0], warp_env0, N, 1, rows, E.boxes);
 }
 
 }  // namespace llq

@@ -440,6 +440,11 @@ struct TailState {            // per env, written by the env's lane 0 (base part
   float pf[3], qp[4], vw[3], ww[3], q[12], qd[12];
 };
 static_assert(sizeof(TailState) <= sizeof(float) * kRowTab, "the hand-over record lives in the row table");
+// termination by orientation (LR:158-179): the body's left axis more than 45 degrees off horizontal, or its up axis more than 60 off vertical
+LLQ_DI bool fallen(const M3& R) {
+  const float left_z = R.a02 * R.a10 - R.a12 * R.a00;
+  return left_z > 0.70710678118654752f || left_z < -0.70710678118654752f || R.a22 < 0.5f;
+}
 template <int ENV>
 LLQ_DI void step_tail(const EnvArrays& E, const MocapDev& mc, const StepParams& P, const ModelConst& M, float* s_new, const float* s_hist,
                       const TailState& T, const float* act_src, float* obs2, long long obs2_ld, int* winner, unsigned long long seed, long long gid0,
@@ -464,28 +469,22 @@ LLQ_DI void step_tail(const EnvArrays& E, const MocapDev& mc, const StepParams& 
   const bool wr = valid;
   const LegConst& L = M.leg[k];
   const Q4 qI = Q4{M.base.qI[0], M.base.qI[1], M.base.qI[2], M.base.qI[3]};
-  Q4 qb;
+  const Q4 qb = qmul(qp, qI);                          // back to the pybullet (inertial-frame) convention
   PairState PS = {0, 0, 1, 0, 0.0, 0.0};
   if (ENV == 0) {
-    qb = qmul(qp, qI);                                 // back to the pybullet (inertial-frame) convention
     float* snew = s_new + el * kNewObs;
     ObsCtx oc = build_obs_new(mc, P, M, k, clip, frame_id, frame_frac, px, py, pz, qb, vw, ww, q, qd, snew);
 #pragma unroll
-    for (int t = 0; t < 3; t++) snew[kPropDim + 3 * k + t] = act_src[3 * k + t];
+    for (int t = 0; t < 3; t++) snew[kSAct + 3 * k + t] = act_src[3 * k + t];
     // reward (PLE:350-426)
     float djp = 0.f, djv = 0.f;
 #pragma unroll
     for (int t = 0; t < 3; t++) { float a = q[t] - oc.kq[t], b = qd[t] - oc.kqd[t]; djp = fmaf(a, a, djp); djv = fmaf(b, b, djv); }
-    V3 fd, fk;
-    {
-      M3 Rp = qmat(qp);
-      V3 f = mul(Rp, foot_in_base(L, q[0], q[1], q[2]));
-      fd = V3{(float)px + f.x, (float)py + f.y, (float)pz + f.z};
-      Q4 kqp = qmul(qnormalize(oc.kb.q), qconj(qI));
-      V3 g = mul(qmat(kqp), foot_in_base(L, oc.kq[0], oc.kq[1], oc.kq[2]));
-      // difference of foot positions, formed in double for the base offset
-      fk = V3{(float)(oc.kb.px - px) + g.x - f.x, (float)(oc.kb.py - py) + g.y - f.y, (float)(oc.kb.pz - pz) + g.z - f.z};
-    }
+    V3 f;
+    const V3 fd = foot_world(L, qp, q, px, py, pz, &f);
+    const V3 g = mul(qmat(qmul(qnormalize(oc.kb.q), qconj(qI))), foot_in_base(L, oc.kq[0], oc.kq[1], oc.kq[2]));
+    // difference of foot positions, formed in double for the base offset
+    const V3 fk = V3{(float)(oc.kb.px - px) + g.x - f.x, (float)(oc.kb.py - py) + g.y - f.y, (float)(oc.kb.pz - pz) + g.z - f.z};
     float dee = dot(fk, fk);
     djp = gsum4(djp); djv = gsum4(djv); dee = gsum4(dee);
     float dpx = (float)(px - oc.kb.px), dpy = (float)(py - oc.kb.py), dpz = (float)(pz - oc.kb.pz);
@@ -495,10 +494,8 @@ LLQ_DI void step_tail(const EnvArrays& E, const MocapDev& mc, const StepParams& 
     float angle = norm3(q_rotvec(qnormalize(qmul(q2, qconj(q1)))));
     float rew = P.w_jp * expf(-1.0f * djp) + P.w_jv * expf(-0.1f * djv) + P.w_ee * expf(-40.0f * dee) +
                 P.w_pose * expf(-20.0f * dp - 10.0f * angle * angle) + P.w_vel * expf(-2.0f * dot(dvl3, dvl3) - 0.2f * dot(dva3, dva3));
-    // termination (PLE:337-348, LR:158-179, ML:168-172)
-    M3 Rq = qmat(q1);
-    float left_z = Rq.a02 * Rq.a10 - Rq.a12 * Rq.a00;
-    bool fall = left_z > 0.70710678118654752f || left_z < -0.70710678118654752f || Rq.a22 < 0.5f;
+    // termination (PLE:337-348, ML:168-172)
+    const bool fall = fallen(qmat(q1));
     int nf = mc.clip_off[clip + 1] - mc.clip_off[clip];
     bool ended = frame_id >= nf - P.margin - 1;
     bool diff = fabsf(angle) > 1.0f || dp > 1.0f;
@@ -538,19 +535,17 @@ LLQ_DI void step_tail(const EnvArrays& E, const MocapDev& mc, const StepParams& 
     const float fix_spd = (float)A[LLQ_AUX_CONTROL_SPD * N + env];
     double total_spd = A[LLQ_AUX_TOTAL_SPD * N + env], max_spd = A[LLQ_AUX_MAX_SPD * N + env];
     PS.flag_draws = (int)A[LLQ_AUX_FLAG_DRAWS * N + env];
-    qb = qmul(qp, qI);
     float* snew = s_new + el * kNewObs;
     const float* spart = s_new + (el ^ 1) * kNewObs;
     sepmc_pair_tail(M, L, k, robot, snew, spart, px, py, pz, qp, qb, vw, ww, q, touch_own, fix_spd, seed, pair_gid, epi, PS);
+    stage_joints(snew, k, q, qd);
 #pragma unroll
-    for (int t = 0; t < 3; t++) { snew[3 * k + t] = q[t]; snew[12 + 3 * k + t] = qd[t]; snew[kPropDim + 3 * k + t] = act_src[3 * k + t]; }
+    for (int t = 0; t < 3; t++) snew[kSAct + 3 * k + t] = act_src[3 * k + t];
     const float spd = sqrtf(vw.x * vw.x + vw.y * vw.y);              // stat_spd (CTG:368-373)
     total_spd += (double)spd;
     if ((double)spd > max_spd) max_spd = (double)spd;
     counter += 1;
-    const M3 Rq = qmat(qnormalize(qb));
-    const float left_z = Rq.a02 * Rq.a10 - Rq.a12 * Rq.a00;
-    int fall = (left_z > 0.70710678118654752f || left_z < -0.70710678118654752f || Rq.a22 < 0.5f) ? 1 : 0;
+    int fall = fallen(qmat(qnormalize(qb))) ? 1 : 0;
     const int fall_other = __shfl_xor_sync(FULL, fall, 4);
     if (robot == 1) fall = fall_other;                                  // only robot 0's fall ends the episode (CTG:462)
     bad = bad || __shfl_xor_sync(FULL, bad ? 1 : 0, 4) != 0;
@@ -561,11 +556,7 @@ LLQ_DI void step_tail(const EnvArrays& E, const MocapDev& mc, const StepParams& 
     if (done && tag) rew += (wf0 != 0) == (robot == 0) ? 1.f : -1.f;
     if (bad) rew = 0.f;
     rew_out = rew;
-    V3 fd;
-    {
-      V3 f = mul(qmat(qp), foot_in_base(L, q[0], q[1], q[2]));
-      fd = V3{(float)px + f.x, (float)py + f.y, (float)pz + f.z};
-    }
+    const V3 fd = foot_world(L, qp, q, px, py, pz);
     if (wr) {
       write_robot(E, N, env, k, q, qd, fd, px, py, pz, qb, vw, ww, time);
       if (k == 0) {
@@ -606,29 +597,20 @@ LLQ_DI void step_tail(const EnvArrays& E, const MocapDev& mc, const StepParams& 
       if (ENV == 3) target_angle = atan2(tgy - sy0, tgx - sx0);            // PGE:318-323 (plotting only)
     }
     __syncwarp();                                        // the pose above is read before lane 0 overwrites it below
-    qb = qmul(qp, qI);
     float* snew = s_new + el * kNewObs;
     const Q4 q1 = qnormalize(qb);
     const M3 Rq = qmat(q1);
+    stage_joints(snew, k, q, qd);
 #pragma unroll
-    for (int t = 0; t < 3; t++) { snew[3 * k + t] = q[t]; snew[12 + 3 * k + t] = qd[t]; snew[kPropDim + 3 * k + t] = act_src[3 * k + t]; }
+    for (int t = 0; t < 3; t++) snew[kSAct + 3 * k + t] = act_src[3 * k + t];
     counter += 1;
     const double dx = tgx - px, dy = tgy - py;
     const double plen = sqrt(dx * dx + dy * dy);
     if (k == 0) {
-      V3 wl = tmul(Rq, ww), vl = tmul(Rq, vw);
-      snew[24] = wl.x; snew[25] = wl.y; snew[26] = wl.z; snew[27] = vl.x; snew[28] = vl.y; snew[29] = vl.z;
-      snew[30] = Rq.a20; snew[31] = Rq.a21; snew[32] = Rq.a22;
-      snew[45] = Rq.a00; snew[46] = Rq.a01; snew[47] = Rq.a02; snew[48] = Rq.a10; snew[49] = Rq.a11; snew[50] = Rq.a12;
-      snew[51] = Rq.a20; snew[52] = Rq.a21; snew[53] = Rq.a22;
-      snew[54] = (float)px; snew[55] = (float)py; snew[56] = (float)pz;
-      V3 dd = tmul(Rq, V3{(float)dx, (float)dy, (float)(0.0 - pz)});
-      float n2_ = sqrtf(dd.x * dd.x + dd.y * dd.y);
-      snew[57] = dd.x / n2_; snew[58] = dd.y / n2_; snew[59] = target_spd;
-      snew[60] = (float)sqrt(px * px + py * py + pz * pz);
+      stage_pose(snew, Rq, tmul(Rq, ww), tmul(Rq, vw), V3{(float)px, (float)py, (float)pz});
+      stage_target(snew, Rq, px, py, pz, tgx, tgy, target_spd);
     }
-    const float left_z = Rq.a02 * Rq.a10 - Rq.a12 * Rq.a00;
-    const bool fall = left_z > 0.70710678118654752f || left_z < -0.70710678118654752f || Rq.a22 < 0.5f;
+    const bool fall = fallen(Rq);
     const bool reach = plen < 0.5, timeup = counter >= P.max_steps;
     const float ux = (float)(dx / plen), uy = (float)(dy / plen);
     const float spd = fabsf(vw.x * ux + vw.y * uy);
@@ -649,11 +631,7 @@ LLQ_DI void step_tail(const EnvArrays& E, const MocapDev& mc, const StepParams& 
     if (bad || !isfinite(rew)) { rew = 0.f; bad = true; }
     done = fall || timeup || reach || bad;
     rew_out = rew;
-    V3 fd;
-    {
-      V3 f = mul(qmat(qp), foot_in_base(L, q[0], q[1], q[2]));
-      fd = V3{(float)px + f.x, (float)py + f.y, (float)pz + f.z};
-    }
+    const V3 fd = foot_world(L, qp, q, px, py, pz);
     if (wr) {
       write_robot(E, N, env, k, q, qd, fd, px, py, pz, qb, vw, ww, time);
       if (k == 0) {
@@ -708,7 +686,7 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
   }
   __pipeline_commit();
   const int warp_env0 = blockIdx.x * EPB + ((tid >> 5) << 1);
-  prefetch_history<ENV, 2>(E.obs, &s_hist[(tid >> 5) << 1][0], warp_env0, N);
+  prefetch_history<ENV, 2>(E.obs, s_hist[(tid >> 5) << 1], warp_env0, N);
   __pipeline_commit();
   __pipeline_wait_prior(1);              // model constants have landed; the history copy stays in flight
   __syncthreads();
@@ -780,7 +758,7 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
   int n_cand = 0;
   float* s_cand = nullptr;
   if (ENV == 3) {
-    s_cand = &s_new[el][0];                            // the staging row is free until the tail: 8 x 6 floats
+    s_cand = s_new[el];                            // the staging row is free until the tail: 8 x 6 floats
     const float* bxs = E.boxes + (size_t)env * (6 * kMaxBoxes);
     // reach of the robot's spheres from the base reference point: hip offset 0.195 + leg 0.48 in x, 0.15 + 0.05 in y, plus the
     // travel during the step (<= 0.06 m at 3 m/s) -> 0.8 m per axis (0.6 missed hind feet stretched backwards over a hurdle)
@@ -1065,8 +1043,8 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
     }
     // ---------------- SEPMC: getContactPoints() (CTG:426-456) = manifolds of the last sub-step, built on its pre-step poses
     if (ENV == 2 && sub == P.substeps - 1) {
-      float* srow = &s_new[el][0];
-      const float* prow = &s_new[el ^ 1][0];
+      float* srow = s_new[el];
+      const float* prow = s_new[el ^ 1];
       const V3 pw = V3{(float)px, (float)py, (float)pz};
       const float* lk = linktab + 24 * k;
       const float c1 = lk[0], s1 = lk[1], c2 = lk[10], s2 = lk[11], c23 = lk[18], s23 = lk[19];
@@ -1076,10 +1054,9 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
       const V3 hp_ = pw + mul(R, p1), ft = pw + mul(R, fb);
       const V3 c0 = pw + mul(R, ld3(M.corner[2 * k])), c1_ = pw + mul(R, ld3(M.corner[2 * k + 1]));
       if (i == 0) {
-        float* o = srow + 18 * k;
-        o[0] = ft.x; o[1] = ft.y; o[2] = ft.z; o[3] = wh.x; o[4] = wh.y; o[5] = wh.z; o[6] = hp_.x; o[7] = hp_.y; o[8] = hp_.z;
-        o[9] = c0.x; o[10] = c0.y; o[11] = c0.z; o[12] = c1_.x; o[13] = c1_.y; o[14] = c1_.z;
-        if (k < 2) { const V3 hd = pw + mul(R, V3{M.handle[k][0], M.handle[k][1], M.handle[k][2]}); o[15] = hd.x; o[16] = hd.y; o[17] = hd.z; }
+        float* o = srow + kSContactRec * k;
+        st3(o, ft); st3(o + 3, wh); st3(o + 6, hp_); st3(o + 9, c0); st3(o + 12, c1_);
+        if (k < 2) st3(o + 15, pw + mul(R, V3{M.handle[k][0], M.handle[k][1], M.handle[k][2]}));
       }
       __syncwarp();
       const float fx = (float)PS.flag_x, fy = (float)PS.flag_y;
@@ -1088,7 +1065,7 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
       bool tg = false;
 #pragma unroll 1
       for (int j = 0; j < 4; j++) {
-        const float* pj = prow + 18 * j;
+        const float* pj = prow + kSContactRec * j;
         const float rj[6] = {M.leg[j].foot_r, M.wheel_r[j], M.hip_r[j], 0.f, 0.f, M.handle[j & 1][3]};
 #pragma unroll
         for (int t = 0; t < 6; t++) {
@@ -1440,13 +1417,13 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
     const int tsrc = tel < EPB ? tel : EPB - 1;
     const int tenv_raw = blockIdx.x * EPB + tsrc;
     const float* tbase = s_env_dyn + tsrc * kEnvFloats;
-    step_tail<ENV>(E, mc, P, M, &s_new[0][0], &s_hist[0][0], *reinterpret_cast<const TailState*>(tbase + (rowtab - linktab)),
+    step_tail<ENV>(E, mc, P, M, s_new[0], s_hist[0], *reinterpret_cast<const TailState*>(tbase + (rowtab - linktab)),
                         tbase + (envtab - linktab) + 44, obs2, obs2_ld, winner, seed, gid0, record, tel, tk, tenv_raw < N ? tenv_raw : N - 1, tval);
   }
   // ---- observation rows (history shift + new prop / action / future; EPMC / SEPMC: the 778 perception rays are cast while the row is
   // written): every warp of the CTA emits the rows of its own two envs, coalesced
   __syncthreads();
-  emit_obs_rows<ENV, 2>(E.obs, obs2, obs2_ld, &s_new[(tid >> 5) << 1][0], &s_hist[(tid >> 5) << 1][0], warp_env0, N, 0, 0x3u, E.boxes);
+  emit_obs_rows<ENV, 2>(E.obs, obs2, obs2_ld, s_new[(tid >> 5) << 1], s_hist[(tid >> 5) << 1], warp_env0, N, 0, 0x3u, E.boxes);
 #ifdef LLQ16_TIMING
   T16_MARK(4);
   t16_[7] = clock64() - t16_s;
