@@ -106,7 +106,9 @@ extern "C" {
 #define LLQ_F_KIN_STATE   7  /* float   [N,37]  kinematic (mocap) robot state (PLE:217-218) -- get only */
 #define LLQ_F_SAMPLE_PROB 8  /* double  [n_clips] prioritized sampling probabilities (PLE:239-240) */
 #define LLQ_F_AVG_REWARD  9  /* double  [n_clips] PLE._avg_reward_sum (PLE:236) */
-#define LLQ_F_EPISODE_ID  10 /* int64   [N]     per-env episode counter (RNG stream position) */
+#define LLQ_F_EPISODE_ID  10 /* int64   [N]     per-env episode counter (RNG stream position).  SEPMC: robot 0's id keys every
+                                                   draw of its pair, and a reset writes robot 0's id + 1 to both robots; unequal ids
+                                                   in a pair are accepted, robot 1's is ignored */
 #define LLQ_F_FOOT_POS    11 /* float   [N,12]  world positions of the 4 foot links after the last step (LR:199-205) -- get only */
 #define LLQ_F_AUX         13 /* double  [N,18]  EPMC bookkeeping (LLQ_AUX_DIM): counters, joystick target, push randomiser, friction */
 #define LLQ_F_OB_ID       14 /* int32   [N]     PMC hurdle: index of the active plate within the clip's plate list (PLE:179,264-265) */

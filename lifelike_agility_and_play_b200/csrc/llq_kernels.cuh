@@ -842,7 +842,7 @@ __global__ void __launch_bounds__(kResetBlock) pmc_reset_kernel(EnvArrays E, Moc
     // ---------------- SEPMC reset (CTG:261-304, 204-230); draws keyed by the pair: stream 1 = [fix_spd, with_flag, friction, x0 |
     // y0, x1, y1, yaw0 | yaw1, flag x, flag y]
     const int robot = env & 1;
-    const long long ep = E.episode[env];
+    const long long ep = E.episode[env & ~1];                        // the pair's episode is robot 0's; both robots get ep + 1
     const long long gid = RP.gid0 + (env & ~1);
     double u0[4], u1[4], u2[4];
     stream_uniforms(RP.seed, gid, ep, 1, 0, u0);

@@ -461,7 +461,7 @@ LLQ_DI void step_tail(const EnvArrays& E, const MocapDev& mc, const StepParams& 
 #pragma unroll
   for (int t = 0; t < 3; t++) { q[t] = T.q[3 * k + t]; qd[t] = T.qd[3 * k + t]; }
   const int clip = ENV == 0 ? E.clip[env] : 0;
-  const long long epi = ENV != 0 ? E.episode[env] - 1 : 0;
+  const long long epi = ENV != 0 ? E.episode[ENV == 2 ? env & ~1 : env] - 1 : 0;   // SEPMC: the pair's id is robot 0's
   const int robot = env & 1;
   const long long pair_gid = gid0 + (env & ~1);
   bool done = false;
@@ -548,7 +548,9 @@ LLQ_DI void step_tail(const EnvArrays& E, const MocapDev& mc, const StepParams& 
     int fall = fallen(qmat(qnormalize(qb))) ? 1 : 0;
     const int fall_other = __shfl_xor_sync(FULL, fall, 4);
     if (robot == 1) fall = fall_other;                                  // only robot 0's fall ends the episode (CTG:462)
-    bad = bad || __shfl_xor_sync(FULL, bad ? 1 : 0, 4) != 0;
+    // the shuffle stands on its own: inside `bad || ...` the lanes of a bad robot would skip it and the warp would wait forever
+    const int bad_other = __shfl_xor_sync(FULL, bad ? 1 : 0, 4);
+    bad = bad || bad_other != 0;
     done = fall != 0 || counter >= P.max_steps || tag || bad;
     // rewards (CTG:640-652, 412-419): +-1 on a flag switch, +-1 on a tag; with_flag after the switch
     const int wf0 = robot == 0 ? PS.with_flag : 1 - PS.with_flag;       // does robot 0 hold the flag
@@ -751,7 +753,7 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
     push_count = (int)A[LLQ_AUX_PUSH_COUNT * N + env];
     pf[0] = (float)A[LLQ_AUX_PUSH_F * N + env]; pf[1] = (float)A[(LLQ_AUX_PUSH_F + 1) * N + env]; pf[2] = (float)A[(LLQ_AUX_PUSH_F + 2) * N + env];
     mu_env = P.mu_ground * (float)A[LLQ_AUX_FOOT_FRICTION * N + env]; push_draws = (int)A[LLQ_AUX_PUSH_DRAWS * N + env];
-    epi = E.episode[env] - 1;                             // streams of the running episode (the reset advanced the counter)
+    epi = E.episode[ENV == 2 ? env & ~1 : env] - 1;       // streams of the running episode (the reset advanced the counter); SEPMC: robot 0's
     if (ENV == 2) { PS.flag_x = A[LLQ_AUX_FLAG_X * N + env]; PS.flag_y = A[LLQ_AUX_FLAG_Y * N + env]; }
   }
   // ---- EPMC corridor: the boxes the robot can reach during this step -> shared memory (<= kMaxCand per env)

@@ -1552,6 +1552,7 @@ void sepmc_step(llq_engine& E, Env& a, Env& b, int64_t gid, const float* act_a, 
   if (*done && pc.tag) {
     if (a.with_flag) { rew2[0] += 1.0; rew2[1] -= 1.0; } else { rew2[0] -= 1.0; rew2[1] += 1.0; }
   }
+  if (!ok) rew2[0] = rew2[1] = 0.0;                                   // a bad step pays nothing, as in PMC and EPMC
   a.reward_sum += rew2[0]; b.reward_sum += rew2[1];
 }
 
