@@ -117,7 +117,8 @@ extern "C" {
 #define LLQ_F_NBOX        16 /* int32   [N]      number of valid boxes */
 #define LLQ_F_DECISION_MARGIN 12 /* float [N]   CPU oracle only, get only: smallest distance to a discontinuous branch taken during
                                    the last step: min(|q-limit|) over joints [rad], min(|dist-contact_breaking|) over the collision spheres [m], and -- where a
-                                   sphere touches two statics at once -- the depth difference that decides which one owns its manifold point [m].
+                                   sphere touches two statics at once -- the depth difference that decides which one owns its manifold point [m];
+                                   under knee_contacts = 1, where a leg's foot and knee wheel both touch, their depth difference (the deeper one is kept) [m].
                                    Parity tests use it to tell rounding noise from a flipped joint-limit / contact decision. */
 
 typedef struct llq_config {

@@ -518,8 +518,8 @@ bool physics_substep(llq_engine& E, Env& e, const double* tau, int64_t* n_contac
       double dpi = dot(pn[pi], cw) - pd[pi] - sp.r;
       if (dpi < dist) { second = dist; dist = dpi; nrm = pn[pi]; } else second = std::min(second, dpi);
     }
-    // EPMC corridor: sphere vs every static box (walls, hurdles, bars, cubes); still one contact per foot, the deepest.
-    // The auxiliary edge cylinders (BSE:43-100) and every non-foot link are not collided (DESIGN.md 5).
+    // EPMC corridor: sphere vs every static box (walls, hurdles, bars, cubes), then the auxiliary edge cylinders below; one contact
+    // per sphere, the deepest.  Under knee_contacts 0 / 1 only the feet meet walls, boxes and cylinders; under 2 every sphere does.
     for (int b = 0; b < (statics ? e.n_boxes : 0); b++) {
       const double* bx = e.boxes[b];
       const double p[3] = {cw.x - bx[0], cw.y - bx[1], cw.z - bx[2]};
@@ -565,8 +565,10 @@ bool physics_substep(llq_engine& E, Env& e, const double* tau, int64_t* n_contac
     for (int leg = 0; leg < 4; leg++) {
       int best = -1;
       for (int ci = 0; ci < nc; ci++)
-        if (contacts[ci].sphere == leg || contacts[ci].sphere == 4 + leg)
+        if (contacts[ci].sphere == leg || contacts[ci].sphere == 4 + leg) {
+          if (best >= 0) e.margin = std::min(e.margin, std::fabs(contacts[ci].dist - contacts[best].dist));   // which of the two wins
           if (best < 0 || contacts[ci].dist < contacts[best].dist) best = ci;
+        }
       for (int ci = 0; ci < nc; ci++)
         if ((contacts[ci].sphere == leg || contacts[ci].sphere == 4 + leg) && ci != best) e.warm[contacts[ci].sphere] = 0.0;
       if (best >= 0) kept[nk++] = contacts[best];

@@ -71,7 +71,8 @@ def quat_from_rpy(roll, pitch, yaw):
 
 # ---------------------------------------------------------------------------------------------------------------- statics
 def _box_dist(cw, b):
-    """clearance of sphere centres cw (n, 3) from box b (centre, half extents) and the outward normal, as the engines compute it"""
+    """clearance of sphere centres cw (n, 3) from box b (centre, half extents), the outward normal as the engines compute it, and --
+    for a centre inside the box -- how much deeper the second-nearest face lies than the one it leaves through (inf outside)"""
     p = cw - b[:3]
     c = np.clip(p, -b[3:6], b[3:6])
     v = p - c
@@ -79,20 +80,24 @@ def _box_dist(cw, b):
     inside = ln == 0.0
     n = v / np.where(inside, 1.0, ln)[:, None]
     d = ln.copy()
+    face_margin = np.full(len(cw), np.inf)
     if inside.any():                                   # centre inside: leave through the nearest face
         depth = np.concatenate([b[3:6] - p, b[3:6] + p], axis=1)[inside]
         f = np.argmin(depth, axis=1)
         d[inside] = -depth[np.arange(len(f)), f]
         nn = np.zeros((len(f), 3)); nn[np.arange(len(f)), f % 3] = np.where(f < 3, 1.0, -1.0)
         n[inside] = nn
-    return d, n
+        face_margin[inside] = np.diff(np.sort(depth, axis=1)[:, :2], axis=1)[:, 0]
+    return d, n, face_margin
 
 
 class Statics:
     """The static shapes a robot's spheres collide with: the ground, the SEPMC arena walls, the boxes of an EPMC corridor (walls
-    first) with the two auxiliary edge cylinders of every box after the walls (tops of hurdles and cubes, bottoms of bars)."""
+    first) with the two auxiliary edge cylinders of every box after the walls (tops of hurdles and cubes, bottoms of bars).
+    rule = llq_config.knee_contacts: the spheres are the first 4 (0: feet), 8 (1: feet, knee wheels) or all 32 (2) rows of SPHERES;
+    under rules 0 and 1 only the feet meet walls, boxes and cylinders."""
 
-    def __init__(self, walls=False, boxes=None, aux_r=0.0, element=0):
+    def __init__(self, walls=False, boxes=None, aux_r=0.0, element=0, rule=2):
         self.walls = walls
         self.boxes = np.zeros((0, 6)) if boxes is None else np.asarray(boxes, np.float64).reshape(-1, 6)
         self.cyl = []
@@ -100,31 +105,44 @@ class Statics:
             for b in self.boxes[2:]:
                 for side in (-1, 1):
                     self.cyl.append((b[0] + side * b[3], b[1], b[2] + (-b[5] if element == 2 else b[5]), b[4], aux_r))
+        self.element, self.rule = element, rule
+        self.ns = {0: 4, 1: 8, 2: len(SPHERES)}[rule]
+        self.radius = RADIUS[:self.ns]
+        self.touch = np.arange(self.ns) < (self.ns if rule == 2 else 4)
 
     def shapes(self, cw):
-        """per static: (clearance (n,), normal (n, 3), kind) with kind 0 ground / plane, 1 box, 2 cylinder"""
-        out = [(cw[:, 2] - RADIUS, np.tile([0.0, 0.0, 1.0], (len(cw), 1)), 0)]
+        """per static: (clearance (n,), normal (n, 3), kind, inside-face margin (n,)) with kind 0 ground / plane, 1 box, 2 cylinder;
+        the clearance from walls, boxes and cylinders is given for every sphere, including those the rule keeps from them"""
+        R = self.radius
+        none = np.full(len(cw), np.inf)
+        out = [(cw[:, 2] - R, np.tile([0.0, 0.0, 1.0], (len(cw), 1)), 0, none)]
         if self.walls:
             for n in ((-1, 0, 0), (1, 0, 0), (0, -1, 0), (0, 1, 0)):
                 n = np.array(n, np.float64)
-                out.append((cw @ n + WALL_IN - RADIUS, np.tile(n, (len(cw), 1)), 0))
+                out.append((cw @ n + WALL_IN - R, np.tile(n, (len(cw), 1)), 0, none))
         for b in self.boxes:
-            d, n = _box_dist(cw, b)
-            out.append((d - RADIUS, n, 1))
+            d, n, fm = _box_dist(cw, b)
+            out.append((d - R, n, 1, fm))
         for x, y, z, hy, r in self.cyl:
             dx, dz = cw[:, 0] - x, cw[:, 2] - z
             ln = np.hypot(dx, dz)
             beside = np.abs(cw[:, 1] - y) > hy
-            d = np.where(beside | (ln == 0), np.inf, ln - r - RADIUS)
+            d = np.where(beside | (ln == 0), np.inf, ln - r - R)
             n = np.stack([dx, np.zeros_like(dx), dz], 1) / np.where(ln == 0, 1.0, ln)[:, None]
-            out.append((d, n, 2))
+            out.append((d, n, 2, none))
         return out
 
+    def off_ground(self, d):
+        """clearances from a wall, box or cylinder as the rule sees them: inf for the spheres it keeps away"""
+        return np.where(self.touch, d, np.inf)
+
     def clearance(self, cw):
-        """(dist, second, normal, owner kind, owner index) per sphere: the owner is the first static with the smallest clearance
-        (index 0 = the ground)"""
+        """(dist, second, normal, owner kind, owner index, inside-face margin, clearance from the nearest wall / box / cylinder
+        ignoring the rule) per sphere: the owner is the first static with the smallest clearance (index 0 = the ground)"""
         sh = self.shapes(cw)
         D = np.stack([s[0] for s in sh])
+        raw = D[1:].min(axis=0) if len(D) > 1 else np.full(len(cw), np.inf)
+        D[1:] = np.where(self.touch, D[1:], np.inf)
         o = np.argmin(D, axis=0)
         idx = np.arange(cw.shape[0])
         dist = D[o, idx]
@@ -132,21 +150,40 @@ class Statics:
         second = D2.min(axis=0)
         normal = np.stack([s[1] for s in sh])[o, idx]
         kind = np.array([s[2] for s in sh])[o]
-        return dist, second, normal, kind, o
+        fm = np.stack([s[3] for s in sh])[o, idx]
+        return dist, second, normal, kind, o, fm, raw
 
 
 # ---------------------------------------------------------------------------------------------------------------- decisions
+LEG_CASES = ("foot_deeper", "wheel_deeper", "wheel_alone", "foot_alone")
+
+
 def decisions(state, statics):
     """Every discrete decision of one sub-step on `state` (fp64 arithmetic on the values as given): per sphere contact / owner /
-    normal, per joint the limit row and its split-impulse side.  Returns a dict with the counts the engines solve and the margin."""
+    normal / the face a centre inside a box leaves through, per joint the limit row and its split-impulse side, and under rule 1 per
+    leg which of foot and knee wheel keeps the leg's one contact.  Returns a dict with the counts the engines solve and the margins."""
     st = np.asarray(state, np.float64)
-    cw = sphere_offsets(st[3:7], st[13:25]) + st[0:3]
-    dist, second, normal, kind, owner = statics.clearance(cw)
+    cw = sphere_offsets(st[3:7], st[13:25])[:statics.ns] + st[0:3]
+    dist, second, normal, kind, owner, face_m, raw = statics.clearance(cw)
     contact = dist < BREAKING
     m = np.abs(dist - BREAKING).min()
     close = second < BREAKING + DELTA_C
     if close.any():
         m = min(m, (second - dist)[close].min())
+    inside = contact & (kind == 1) & (dist + statics.radius < 0)        # centre inside a box
+    if inside.any():
+        m = min(m, face_m[inside].min())
+    legs, m_r = [None] * 4, np.inf
+    if statics.rule == 1:                              # one contact per leg, the deeper of foot and wheel (the foot wins ties)
+        for l in range(4):
+            f, w = l, 4 + l
+            if contact[f] and contact[w]:
+                m_r = min(m_r, abs(dist[f] - dist[w]))
+                legs[l] = "wheel_deeper" if dist[w] < dist[f] else "foot_deeper"
+                contact[f if dist[w] < dist[f] else w] = False
+            elif contact[w] or contact[f]:
+                legs[l] = "wheel_alone" if contact[w] else "foot_alone"
+    kept = np.flatnonzero(contact)
     general = contact & (kind != 0)                    # box / cylinder normals go through btPlaneSpace1's two branches
     nz = np.abs(normal[:, 2])
     m_n = np.abs(nz - np.sqrt(0.5))[general].min() if general.any() else np.inf
@@ -156,12 +193,16 @@ def decisions(state, statics):
     mq = min(np.abs(q - LOWER).min(), np.abs(UPPER - q).min())
     if viol.any():
         mq = min(mq, np.abs(pen[viol] - SPLIT_PEN).min())
-    return dict(nc=int(contact.sum()), nl=int(viol.sum()), contact=contact, n_off_ground=int((contact & (owner != 0)).sum()), pen=pen[viol], margin_c=m, margin_q=mq, margin_n=m_n,
-                nz=nz[general])
+    # a sphere the rule keeps from walls and boxes, within the breaking distance of one and clear of the ground, both by DELTA_C
+    ignored = ~statics.touch & (raw < BREAKING - DELTA_C) & (cw[:, 2] - statics.radius >= BREAKING + DELTA_C)
+    return dict(nc=int(contact.sum()), nl=int(viol.sum()), contact=contact, n_off_ground=int((contact & (owner != 0)).sum()), pen=pen[viol],
+                margin_c=m, margin_q=mq, margin_n=m_n, margin_r=m_r, nz=nz[general], normal=normal[general], kind=kind[general],
+                inside=int(inside.sum()), legs=legs, ignored=int(ignored.sum()),
+                leg_order=bool(statics.rule == 1 and list(kept) != sorted(kept, key=lambda s: s % 4)))
 
 
 def clear(dec):
-    return dec["margin_c"] >= DELTA_C and dec["margin_q"] >= DELTA_Q and dec["margin_n"] >= DELTA_N
+    return dec["margin_c"] >= DELTA_C and dec["margin_q"] >= DELTA_Q and dec["margin_n"] >= DELTA_N and dec["margin_r"] >= DELTA_C
 
 
 # ---------------------------------------------------------------------------------------------------------------- sampling
@@ -203,19 +244,51 @@ def _place(rng, off, shape_fn, direction, k, ref, lo=-0.05):
 
 def design(rng, statics, family="stand", n_viol=0, k_ground=0, target=None, tilt=0.15):
     """One designed state (float32 values) or None.  target: None (ground only), ('wall', k), ('top', box, k), ('face', box, k),
-    ('cyl', index, k)."""
+    ('cyl', index, k), ('under', bar, k), ('under_cyl', index, k); with '_any' appended to the name the k-th closest sphere is
+    counted among all spheres, also those the contact rule keeps from walls and boxes."""
     q = _joint_angles(rng, family, n_viol).astype(np.float32).astype(np.float64)
     quat = quat_from_rpy(tilt * rng.standard_normal(), tilt * rng.standard_normal(), rng.uniform(-np.pi, np.pi))
     quat = (quat / np.linalg.norm(quat)).astype(np.float32).astype(np.float64)
-    off = sphere_offsets(quat, q)
-    ground = lambda c: c[:, 2] - RADIUS
+    off = sphere_offsets(quat, q)[:statics.ns]
+    R, ring = statics.radius, statics.off_ground
+    if target is not None and target[0].endswith("_any"):   # place the k-th closest of all spheres, also those the rule keeps away
+        target, ring = (target[0][:-4],) + tuple(target[1:]), (lambda d: d)
+    ground = lambda c: c[:, 2] - R
     ez = np.array([0.0, 0.0, 1.0])
     p = np.zeros(3)
     if target is not None and target[0] == "top":
         b = statics.boxes[target[1]]
         p = np.array([b[0] + rng.uniform(-0.5, 0.5) * b[3], b[1] + rng.uniform(-0.5, 0.5) * b[4], b[2] + b[5]])   # a point of the top face
-        box = lambda c: _box_dist(c, b)[0] - RADIUS
+        box = lambda c: ring(_box_dist(c, b)[0] - R)
         p = _place(rng, off, box, ez, target[2], p)
+    elif target is not None and target[0] in ("under", "under_cyl"):
+        # on the ground below a bar, crouched until the k-th closest sphere meets the bar's bottom face (n = -z) or one of its
+        # bottom-edge cylinders
+        if target[0] == "under":
+            b = statics.boxes[target[1]]
+            xy = np.array([b[0] + rng.uniform(-0.3, 0.3), b[1] + rng.uniform(-0.5, 0.5) * b[4], 0.0])
+            box = lambda c: ring(_box_dist(c, b)[0] - R)
+        else:
+            x, y, z, hy, r = statics.cyl[target[1]]
+            xy = np.array([x + rng.uniform(-0.35, 0.35), y + rng.uniform(-0.5, 0.5) * hy, 0.0])
+            box = lambda c: ring(np.where(np.abs(c[:, 1] - y) > hy, np.inf, np.hypot(c[:, 0] - x, c[:, 2] - z) - r - R))
+        kb = target[2]
+        tb = BREAKING - rng.uniform(DELTA_C + 5e-4, 0.006)
+        tg = BREAKING - rng.uniform(DELTA_C + 5e-4, 0.006)
+        crouch = np.tile([0.0, -1.0, 2.0], 4)
+
+        def at(s):
+            qs = np.clip(q + s * crouch, LOWER + DELTA_Q + 1e-3, UPPER - DELTA_Q - 1e-3).astype(np.float32).astype(np.float64)
+            o = sphere_offsets(quat, qs)[:statics.ns]
+            lift = tg - np.sort(ground(o + xy))[max(k_ground, 1) - 1]
+            return qs, xy + lift * ez, np.sort(box(o + xy + lift * ez))[kb - 1] - tb
+        lo_s, hi_s = 0.0, 0.7
+        if at(lo_s)[2] > 0 or at(hi_s)[2] < 0:
+            return None
+        for _ in range(30):
+            mid = 0.5 * (lo_s + hi_s)
+            lo_s, hi_s = (mid, hi_s) if at(mid)[2] < 0 else (lo_s, mid)
+        q, p, _ = at(hi_s)
     else:
         if target is not None and target[0] == "face":
             b = statics.boxes[target[1]]
@@ -231,14 +304,16 @@ def design(rng, statics, family="stand", n_viol=0, k_ground=0, target=None, tilt
             p = _place(rng, off, ground, ez, k_ground, p)
         if p is not None and target is not None:
             if target[0] == "wall":
-                p = _place(rng, off, lambda c: WALL_IN - c[:, 0] - RADIUS, np.array([-1.0, 0.0, 0.0]), target[1], p)
+                p = _place(rng, off, lambda c: ring(WALL_IN - c[:, 0] - R), np.array([-1.0, 0.0, 0.0]), target[1], p)
             elif target[0] == "face":
-                box = lambda c: _box_dist(c, b)[0] - RADIUS
+                box = lambda c: ring(_box_dist(c, b)[0] - R)
                 p = _place(rng, off, box, np.array([-1.0, 0.0, 0.0]), target[2], p)
             else:
                 phi = rng.uniform(0.15, np.pi - 0.15)
+                if statics.element == 2:               # a bar's cylinders sit on its bottom edges: approach from below
+                    phi = -phi
                 d = np.array([np.cos(phi), 0.0, np.sin(phi)])
-                cyl = lambda c: np.where(np.abs(c[:, 1] - y) > hy, np.inf, np.hypot(c[:, 0] - x, c[:, 2] - z) - r - RADIUS)
+                cyl = lambda c: ring(np.where(np.abs(c[:, 1] - y) > hy, np.inf, np.hypot(c[:, 0] - x, c[:, 2] - z) - r - R))
                 p = _place(rng, off, cyl, d, target[2], p, lo=0.0)
     if p is None:
         return None
@@ -354,18 +429,33 @@ def ground_batch(rng, statics, kind=0):
     return np.stack([g[0] for g in got]), [g[1] for g in got]
 
 
-def corridor_batch(rng, statics_of, boxes, nbox):
+def corridor_batch(rng, statics_of, boxes, nbox, element=1):
     """EPMC corridor: env i is designed against its own corridor (statics_of(i)) -- on a box top, against a box face, on an edge
-    cylinder, heavy on the ground between the boxes -- 2 CTAs and a ragged third."""
+    cylinder, heavy on the ground between the boxes -- 2 CTAs and a ragged third.  Bars (element 2) have roles of their own, each a
+    robot standing on the ground under a bar with its back touching it: a sphere at the bar's bottom face (n = -z), trunk corners
+    (r = 0) whose centre is inside the bar, a sphere on one of its bottom-edge cylinders (the two sides in turn); and heavy robots on
+    the ground between the bars."""
     n = boxes.shape[0]
     states, decs = [], []
     for i in range(n):
         S = statics_of(i)
         nb = int(nbox[i])
-        role = i % 4
-        for _ in range(200):
+        role = i % (5 if element == 2 else 4)
+        for _ in range(400):
             j = int(rng.integers(2, nb))
-            if role == 0:
+            want = None
+            if element == 2:
+                if role < 2:                           # role 1: a trunk corner's centre inside the bar
+                    kw = dict(family="stand", n_viol=0, tilt=0.1, k_ground=int(rng.integers(1, 5)), target=("under", j, int(rng.integers(1, 3))))
+                    want = (lambda d: d["inside"] == 0 and d["nc"] > d["n_off_ground"] and 1 in d["kind"]) if role == 0 else (lambda d: d["inside"] > 0 and d["nc"] > d["n_off_ground"])
+                elif role < 4:                         # the two bottom-edge cylinders in turn
+                    kw = dict(family="stand", n_viol=0, tilt=0.1, k_ground=int(rng.integers(1, 5)),
+                              target=("under_cyl", 2 * (j - 2) + (i // 5 + role) % 2, int(rng.integers(1, 3))))
+                    want = lambda d: d["nc"] > d["n_off_ground"] > 0 and 2 in d["kind"]
+                else:
+                    kw = dict(family="fold", n_viol=int(rng.integers(3, 8)), k_ground=int(rng.integers(6, 9)), tilt=0.05)
+                    want = lambda d: 3 * min(d["nc"], MAX_CON) + min(d["nl"], MAX_LIM) > 16
+            elif role == 0:
                 kw = dict(family="stand", n_viol=int(rng.integers(0, 3)), target=("top", j, int(rng.integers(1, 5))))
             elif role == 1:
                 kw = dict(family="stand", n_viol=int(rng.integers(0, 3)), k_ground=int(rng.integers(0, 4)), target=("face", j, int(rng.integers(1, 4))))
@@ -373,10 +463,73 @@ def corridor_batch(rng, statics_of, boxes, nbox):
                 kw = dict(family="stand", n_viol=int(rng.integers(0, 2)), tilt=0.4, target=("cyl", 2 * (j - 2) + int(rng.integers(0, 2)), int(rng.integers(1, 3))))
             else:
                 kw = dict(family="fold", n_viol=int(rng.integers(3, 8)), k_ground=int(rng.integers(6, 9)), tilt=0.05, target=("face", j, 1))
+                want = lambda d: 3 * min(d["nc"], MAX_CON) + min(d["nl"], MAX_LIM) > 16
             res = design(rng, S, **kw)
-            if res is not None and (role != 3 or 3 * min(res[1]["nc"], MAX_CON) + min(res[1]["nl"], MAX_LIM) > 16):
+            if res is not None and (want is None or want(res[1])):
                 break
         else:
             raise RuntimeError("no corridor state for env %d (role %d)" % (i, role))
         states.append(res[0]); decs.append(res[1])
+    return np.stack(states), decs
+
+
+LEGACY_FEATURES = {0: ("ground", "off_ground"),
+                   1: ("foot_deeper", "wheel_deeper", "wheel_alone", "leg_order", "ignored", "off_ground")}
+
+
+def features(dec):
+    """the legacy-set categories one designed state reaches"""
+    f = {x for x in dec["legs"] if x is not None}
+    if dec["leg_order"]:
+        f.add("leg_order")
+    if dec["ignored"]:
+        f.add("ignored")
+    if dec["n_off_ground"]:
+        f.add("off_ground")
+    if dec["nc"] > dec["n_off_ground"]:
+        f.add("ground")
+    return f
+
+
+def legacy_batch(rng, statics_of, n, rule, boxes=0):
+    """Rules 0 and 1 (feet; feet and knee wheels, one contact per leg): 3 CTAs, N = n (>= 40).  CTA 0: 6 light robots (<= 12 rows)
+    beside 10 airborne ones -> split16, empty; CTA 1: 8 robots with 17..20 rows (4 contacts, >= 5 limit rows) beside 8 light ones ->
+    borrow; CTA 2 (ragged): airborne robots and env N - 1 with 17..20 rows -> borrow_empty.  The light robots take the categories of
+    LEGACY_FEATURES in turn (against the statics' walls or boxes where there are any: boxes > 2 is the corridor's box count)."""
+    walls = statics_of(0).walls
+    feats = [f for f in LEGACY_FEATURES[rule] if (walls or boxes > 2) or f not in ("ignored", "off_ground")]
+    plan = (["light"] * 6 + ["air"] * 10 + ["mid"] * 8 + ["light"] * 8 + ["air"] * (n - 33) + ["mid"])
+    states, decs, nl_ = [], [], 0
+    for i, role in enumerate(plan):
+        S = statics_of(i)
+        want_f = feats[nl_ % len(feats)] if role == "light" else None
+        nl_ += role == "light"
+        for _ in range(6000):
+            j = int(rng.integers(2, boxes)) if boxes > 2 else 0
+            k = int(rng.integers(1, 4))
+            target = None
+            if want_f in ("ignored", "off_ground"):
+                tail = "_any" if want_f == "ignored" else ""
+                target = ("wall" + tail, k) if walls else (("face" + tail, j, k) if rng.random() < 0.7 else ("top", j, k))
+            if role == "air":
+                kw = dict(family="stand", n_viol=0, k_ground=0)
+            elif role == "mid":
+                kw = dict(family="stand", n_viol=int(rng.integers(5, 9)), k_ground=int(rng.integers(4, S.ns + 1)), tilt=0.1)
+            else:
+                kw = dict(family=("stand", "fold")[int(rng.integers(0, 2))], n_viol=int(rng.integers(0, 2)),
+                          k_ground=int(rng.integers(0 if target else 1, min(7, S.ns + 1))), tilt=0.3, target=target)
+            res = design(rng, S, **kw)
+            if res is None:
+                continue
+            d = res[1]
+            rows = 3 * d["nc"] + d["nl"]
+            if role == "air" and d["nc"] == 0 and d["nl"] == 0:
+                break
+            if role == "mid" and 17 <= rows <= 20:
+                break
+            if role == "light" and 1 <= d["nc"] and rows <= 12 and want_f in features(d):
+                break
+        else:
+            raise RuntimeError("no rule-%d state for env %d (%s, %s)" % (rule, i, role, want_f))
+        states.append(res[0]); decs.append(d)
     return np.stack(states), decs

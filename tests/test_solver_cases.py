@@ -6,7 +6,7 @@ import pytest
 
 import solver_cases as sc
 from lifelike_agility_and_play_b200 import _capi as capi
-from test_golden_epmc import terrain_cfg, terrain_gold
+from test_golden_epmc import EPMC_CFG, GOLD as EPMC_GOLD, terrain_cfg, terrain_gold
 from test_golden_sepmc import SEPMC_CFG
 
 SEED = 20261015
@@ -20,6 +20,9 @@ def kind_cfg(kind, element=1):
     if kind == "sepmc":
         cfg = dict(SEPMC_CFG); cfg.update(base, push_enabled=0, max_steps=1000, friction_hi=1.0)
         return cfg
+    if kind == "epmc":                                 # the flat arena, element 0
+        cfg = dict(EPMC_CFG); cfg.update(base, push_enabled=0, max_steps=1000, friction_hi=1.0)
+        return cfg
     cfg = terrain_cfg(terrain_gold(element)); cfg.update(base, push_enabled=0, max_steps=1000, friction_hi=1.0)
     return cfg
 
@@ -30,6 +33,8 @@ def init_state(kind, element=1):
     if kind == "sepmc":
         from test_golden_sepmc import GOLD
         return np.load(GOLD)["init_state"]
+    if kind == "epmc":
+        return np.load(EPMC_GOLD)["init_state"]
     return terrain_gold(element)["init_state"]
 
 
@@ -42,38 +47,43 @@ def make(lib, kind, n, blob, mocap, element=1, **over):
     return e
 
 
-def corridor_statics(eng, element):
+def corridor_statics(eng, element, rule=2):
     boxes = eng.get(capi.F_BOXES).reshape(eng.n, 36, 6).astype(np.float64)
     nbox = eng.get(capi.F_NBOX)
     aux = kind_cfg("corridor", element)["auxiliary_radius"]
-    return boxes, nbox, (lambda i: sc.Statics(boxes=boxes[i, :nbox[i]], aux_r=aux, element=element))
+    return boxes, nbox, (lambda i: sc.Statics(boxes=boxes[i, :nbox[i]], aux_r=aux, element=element, rule=rule))
 
 
-def designed_batch(kind, oracle_lib, blob, mocap, element=1):
-    """(states [N, 37] float32, per-env decisions) of the batch a kind's GPU test runs; deterministic"""
-    rng = np.random.default_rng(SEED + {"pmc": 0, "sepmc": 1, "corridor": 10 + element}[kind])
+def designed_batch(kind, oracle_lib, blob, mocap, element=1, rule=2):
+    """(states [N, 37] float32, per-env decisions) of the batch a kind's GPU test runs (rule = llq_config.knee_contacts);
+    deterministic"""
+    rng = np.random.default_rng(SEED + {"pmc": 0, "sepmc": 1, "epmc": 20, "corridor": 10 + element}[kind] + 100 * (2 - rule))
     if kind == "corridor":
         eng = make(oracle_lib, kind, 40, blob, mocap, element)
-        boxes, nbox, statics_of = corridor_statics(eng, element)
+        boxes, nbox, statics_of = corridor_statics(eng, element, rule)
         eng.close()
-        return sc.corridor_batch(rng, statics_of, boxes, nbox)
-    return sc.ground_batch(rng, sc.Statics(walls=kind == "sepmc"), kind=2 if kind == "sepmc" else 0)
+        if rule != 2:
+            return sc.legacy_batch(rng, statics_of, 40, rule, boxes=int(nbox.min()))
+        return sc.corridor_batch(rng, statics_of, boxes, nbox, element)
+    S = sc.Statics(walls=kind == "sepmc", rule=rule)
+    if rule != 2:
+        return sc.legacy_batch(rng, lambda i: S, 40, rule)
+    return sc.ground_batch(rng, S, kind=2 if kind == "sepmc" else 0)
 
 
-KINDS = [("pmc", 1), ("sepmc", 1), ("corridor", 1), ("corridor", 3)]
+KINDS = [("pmc", 1), ("sepmc", 1), ("corridor", 1), ("corridor", 3), ("epmc", 0), ("corridor", 2)]
+# the legacy contact sets (llq_config.knee_contacts 0: the feet, 1: feet and knee wheels, one contact per leg)
+LEGACY = [(k, 1, r) for k in ("pmc", "sepmc", "corridor") for r in (0, 1)]
 
 
-@pytest.mark.parametrize("kind,element", KINDS)
-def test_designed_states_take_their_branches_on_the_oracle(kind, element, oracle_lib, blob, small_mocap):
+def oracle_one_by_one(oracle_lib, blob, mocap, kind, element, states, decs, **over):
     """Each designed state alone in a one-env oracle handle (SEPMC: a pair of two copies), one sub-step: the contact and limit rows
-    solved and the rows dropped by the caps are exactly the designed ones, and no decision is within DELTA of its branch."""
-    states, decs = designed_batch(kind, oracle_lib, blob, small_mocap, element)
-    n = len(states)
-    reached = sc.warp_cases([d["nc"] for d in decs], [d["nl"] for d in decs])[1]
+    solved and the rows dropped by the caps are exactly the designed ones, and no decision is within DELTA of its branch.  Returns
+    the smallest oracle decision margin."""
     width = 2 if kind == "sepmc" else 1
     worst = np.inf
-    for i in range(n):
-        e = make(oracle_lib, kind, width, blob, small_mocap, element, global_env_offset=i if kind == "corridor" else 0)
+    for i in range(len(states)):
+        e = make(oracle_lib, kind, width, blob, mocap, element, global_env_offset=i if kind == "corridor" else 0, **over)
         e.set(capi.F_STATE, np.repeat(states[i:i + 1], width, 0)); e.set(capi.F_WARMSTART, np.zeros((width, 32), np.float32))
         c0 = e.counters().copy()
         e.step(np.zeros((width, 12), np.float32))
@@ -85,15 +95,37 @@ def test_designed_states_take_their_branches_on_the_oracle(kind, element, oracle
         worst = min(worst, m)
         assert m >= 0.999 * sc.DELTA_C, (kind, i, m)
         e.close()
-    print("%s: %d designed states, smallest oracle decision margin %.1e; mapping cases of the batch: %s" % (kind, n, worst, sorted(reached)))
+    return worst
+
+
+@pytest.mark.parametrize("kind,element", KINDS)
+def test_designed_states_take_their_branches_on_the_oracle(kind, element, oracle_lib, blob, small_mocap):
+    """Each designed state alone in a one-env oracle handle (SEPMC: a pair of two copies), one sub-step: the contact and limit rows
+    solved and the rows dropped by the caps are exactly the designed ones, and no decision is within DELTA of its branch."""
+    states, decs = designed_batch(kind, oracle_lib, blob, small_mocap, element)
+    reached = sc.warp_cases([d["nc"] for d in decs], [d["nl"] for d in decs])[1]
+    worst = oracle_one_by_one(oracle_lib, blob, small_mocap, kind, element, states, decs)
+    print("%s element %d: %d designed states, smallest oracle decision margin %.1e; mapping cases of the batch: %s" % (
+        kind, element, len(states), worst, sorted(reached)))
 
 
 @pytest.mark.parametrize("kind,element", KINDS)
 def test_designed_batches_reach_every_lane_mapping(kind, element, oracle_lib, blob, small_mocap):
     states, decs = designed_batch(kind, oracle_lib, blob, small_mocap, element)
     mapping, reached = sc.warp_cases([d["nc"] for d in decs], [d["nl"] for d in decs])
-    print("%s: %d envs, cases reached: %s" % (kind, len(states), sorted(reached)))
-    if kind == "corridor":
+    print("%s element %d: %d envs, cases reached: %s" % (kind, element, len(states), sorted(reached)))
+    if kind == "corridor" and element == 2:
+        assert reached & {"two_pass", "borrow", "borrow_empty"}, reached
+        nrm = np.concatenate([d["normal"] for d in decs]); kd = np.concatenate([d["kind"] for d in decs])
+        cyl_nz = np.abs(nrm[kd == 2, 2])
+        # bottom faces (n = -z), corners inside a bar, bottom-edge cylinders on both sides of btPlaneSpace1's branch, both cylinders
+        assert (nrm[kd == 1, 2] == -1).any(), nrm[kd == 1]
+        assert sum(d["inside"] for d in decs) > 0
+        assert (cyl_nz > np.sqrt(0.5)).any() and (cyl_nz < np.sqrt(0.5)).any(), cyl_nz
+        assert (nrm[kd == 2, 0] > 0).any() and (nrm[kd == 2, 0] < 0).any()
+        # every bar robot also stands on the ground
+        assert all(d["nc"] > d["n_off_ground"] for d in decs if d["n_off_ground"])
+    elif kind == "corridor":
         assert reached & {"two_pass", "borrow", "borrow_empty"}, reached
         nz = np.concatenate([d["nz"] for d in decs])
         # box tops (|n.z| = 1) and faces (0), and edge-cylinder / box-edge normals on both sides of btPlaneSpace1's branch
@@ -105,6 +137,28 @@ def test_designed_batches_reach_every_lane_mapping(kind, element, oracle_lib, bl
     if kind != "corridor":
         # limit rows on both sides of the split-impulse threshold, some of them within 1 cm of it on the deep side
         assert (pens > sc.SPLIT_PEN).any() and (pens < sc.SPLIT_PEN - 0.005).any() and ((pens < sc.SPLIT_PEN) & (pens > -0.05)).any()
+
+
+@pytest.mark.parametrize("kind,element,rule", LEGACY)
+def test_legacy_contact_sets_take_their_branches_and_reach_every_category(kind, element, rule, oracle_lib, blob, small_mocap):
+    """knee_contacts 0 and 1: every designed state takes its branches on the oracle (under rule 1 including which of a leg's foot and
+    knee wheel is deeper, by at least DELTA_C), and the batch reaches the lane mappings 4-8 spheres allow and, per env, the
+    categories of solver_cases.LEGACY_FEATURES: foot deeper, wheel deeper, wheel alone, a leg-order index other than the sphere-order
+    one, a knee wheel within the breaking distance of a wall or box that neither engine collides, feet on walls and boxes."""
+    states, decs = designed_batch(kind, oracle_lib, blob, small_mocap, element, rule)
+    reached = sc.warp_cases([d["nc"] for d in decs], [d["nl"] for d in decs])[1]
+    assert {"split16", "borrow", "borrow_empty", "empty"} <= reached, reached
+    got = {}
+    for i, d in enumerate(decs):
+        assert d["nc"] <= 4 and (rule == 1 or d["ignored"] == 0)
+        for f in sc.features(d):
+            got.setdefault(f, []).append(i)
+    want = set(sc.LEGACY_FEATURES[rule]) - (set() if kind != "pmc" else {"ignored", "off_ground"})
+    assert want <= set(got), want - set(got)
+    margin_r = min(d["margin_r"] for d in decs)
+    worst = oracle_one_by_one(oracle_lib, blob, small_mocap, kind, element, states, decs, knee_contacts=rule)
+    print("%s rule %d: %d envs, mapping cases %s; categories (envs): %s; smallest foot-vs-wheel margin %.1e, smallest oracle margin %.1e" % (
+        kind, rule, len(states), sorted(reached), {f: len(v) for f, v in sorted(got.items())}, margin_r, worst))
 
 
 def test_the_mapping_follows_the_documented_rule():
@@ -177,3 +231,223 @@ def test_no_corridor_puts_more_boxes_in_reach_than_the_kernel_keeps(element, ora
             worst = max(worst, int((inx & iny).sum(-1).max()))
     print("element %d: at most %d boxes within the window" % (element, worst))
     assert worst <= KERNEL_MAX_CAND
+
+
+# ---------------------------------------------------------------------------------------------------------------- pushes and clamps
+DYN_KINDS = [("epmc", 0), ("sepmc", 1), ("corridor", 1)]
+DYN_CASES = ("push_in", "push_redraw", "push_after", "pd_clamp", "vel_clamp", "vel_impulse")
+PUSH_MIN = 10.0           # N: the least push the batches keep
+
+
+def _pd_clamps(rng, st, kp, kd, max_tau):
+    """PD target and torque clamps on an airborne state (float32 values changed in place, actions returned):
+      - the thighs of legs 0 / 1 at q = -2.85 +- 0.05 (clear of both stops) with q + a below -3: the target clamp sets the target to
+        -3, and the torque kp (-3 - q) - kd qd (qd within +-1 rad/s) stays inside +-max_tau -- a target clamp at +-pi would saturate it;
+      - the knees of legs 2 / 3 within 0.03..0.06 rad of their upper stop with q + a above +3, and qd (about 15..25 rad/s) such that
+        the torque kp (3 - q) - kd qd is 2..5 Nm inside +max_tau;
+      - every hip torque past +max_tau (legs 0, 2) or -max_tau (legs 1, 3), with joint velocities of 5..15 rad/s against it, so that
+        the joint damping that follows the clamp is not 0."""
+    a = np.clip(0.3 * rng.standard_normal(12), -1, 1)
+    q, qd = st[13:25], st[25:37]
+    for k in range(2):
+        j = 3 * k + 1
+        q[j] = -2.85 + rng.uniform(-0.05, 0.05); qd[j] = rng.uniform(-1, 1)
+        a[j] = -3.0 - q[j] - rng.uniform(0.3, 1.0)
+    for k in (2, 3):
+        j = 3 * k + 2
+        q[j] = sc.UPPER[j] - rng.uniform(0.03, 0.06)
+        qd[j] = (kp * (3.0 - float(np.float32(q[j]))) - max_tau + rng.uniform(2.0, 5.0)) / kd
+        a[j] = 3.0 - q[j] + rng.uniform(0.3, 1.0)
+    for k in range(4):
+        s = 1.0 if k % 2 == 0 else -1.0
+        qd[3 * k] = -s * rng.uniform(5.0, 15.0)
+        a[3 * k] = s * (max_tau + 2.0 + kd * abs(qd[3 * k])) / kp + s * rng.uniform(0.0, 0.3)
+    return a
+
+
+def pd_categories(st, a, kp, kd, max_tau):
+    """per joint: '+target' / '-target' (q + a beyond +-3 by 0.05, the torque from the clamped target inside +-max_tau by 0.5 Nm),
+    '+tau' / '-tau' (the PD torque beyond +-max_tau by 1 Nm)"""
+    q, qd = st[13:25].astype(np.float64), st[25:37].astype(np.float64)
+    tg = np.clip(q + a, -3, 3)
+    tau = kp * (tg - q) - kd * qd
+    cat = np.full(12, "", object)
+    inside = np.abs(tau) < max_tau - 0.5
+    cat[(q + a > 3.05) & inside] = "+target"; cat[(q + a < -3.05) & inside] = "-target"
+    cat[tau > max_tau + 1] = "+tau"; cat[tau < -max_tau - 1] = "-tau"
+    return cat
+
+
+VEL = np.r_[7:13, 25:37]    # the base (linear, angular) and joint velocities of a state row: each clamped to +-max_coord_vel
+
+
+def crossings(before, after, vmax):
+    """per env: velocity entries that start inside the bound by 1e-4 and that the sub-step carries beyond it by 1e-4 (after: the
+    oracle's state with max_coord_vel at 1e9, no rows), and entries that start beyond it"""
+    v0, v1 = np.abs(before[:, VEL].astype(np.float64)), np.abs(after[:, VEL])
+    return ((v0 < vmax - 1e-4) & (v1 > vmax + 1e-4)).sum(1), (v0 > vmax).sum(1)
+
+
+def dynamics_batch(kind, oracle_lib, blob, mocap, element):
+    """Designed pairs of envs (SEPMC: the two robots of a pair), one case of DYN_CASES per pair, in turn: a push inside its window, on
+    the window's first sub-step after an interval redraw, on the first sub-step after the window (airborne robots and robots on the
+    ground alone, decisions as in the solver pin); the PD target and torque clamps (_pd_clamps); velocities within 3 m/s of
+    +-max_coord_vel, some beyond it and some that the sub-step carries across it (airborne, see designed_dynamics); a robot falling at
+    30..60 m/s onto the ground, whose contact impulse drives joint velocities into the bound.  Every state is checked against the
+    statics of its own env (corridor: its own corridor, the robot on the corridor's centre line 8 m before its start).
+    Returns (states, decisions, actions, case per env, the batch handle's llq_config); designed_dynamics adds the F_AUX schedule."""
+    rng = np.random.default_rng(SEED + 50 + {"epmc": 0, "sepmc": 1, "corridor": 2}[kind])
+    npair = 4 * len(DYN_CASES)
+    eng = make(oracle_lib, kind, 2 * npair, blob, mocap, element)
+    cfg = eng.cfg
+    S = sc.Statics(walls=kind == "sepmc")
+    statics_of = corridor_statics(eng, element)[2] if kind == "corridor" else (lambda i: S)
+    eng.close()
+    states, decs, acts, cases = [], [], [], []
+    for p in range(npair):
+        case = DYN_CASES[p % len(DYN_CASES)]
+        for r in range(2):
+            i = len(states)
+            partner = kind == "sepmc" and r == 1 and case.startswith("push")      # the partner of a pushed SEPMC robot
+            name = "light" if case == "vel_impulse" or (case.startswith("push") and r == 1 and not partner) else "air"
+            for _ in range(200):
+                st, d0 = sc.robot(rng, S, name)
+                st = st.copy(); a = np.clip(0.3 * rng.standard_normal(12), -1, 1)
+                if partner:
+                    a = np.zeros(12)
+                elif case == "pd_clamp":
+                    a = _pd_clamps(rng, st, cfg.kp, cfg.kd, cfg.max_tau)
+                    cat = pd_categories(st, a.astype(np.float32), cfg.kp, cfg.kd, cfg.max_tau)
+                    if not ({"+target", "-target", "+tau", "-tau"} <= set(cat)):
+                        continue
+                elif case == "vel_clamp":
+                    pick = rng.random(18) < 0.5
+                    v = np.sign(rng.standard_normal(18)) * (cfg.max_coord_vel + rng.uniform(0.5, 3.0, 18))
+                    st[VEL[pick]] = v[pick]
+                elif case == "vel_impulse":
+                    st[9] = -rng.uniform(30.0, 60.0)
+                if kind == "corridor":
+                    b = statics_of(i).boxes
+                    st[0] -= 8.0; st[1] = 0.5 * (b[0, 1] + b[1, 1]) + rng.uniform(-0.05, 0.05)
+                d = sc.decisions(st, statics_of(i))
+                if sc.clear(d) and (d["nc"], d["nl"], d["n_off_ground"]) == (d0["nc"], d0["nl"], 0):
+                    break
+            else:
+                raise RuntimeError("no %s state for env %d (%s)" % (case, i, kind))
+            states.append(st); decs.append(d); acts.append(a); cases.append(case)
+    return np.stack(states).astype(np.float32), decs, np.stack(acts).astype(np.float32), cases, cfg
+
+
+def push_aux(eng, cases, rng_seed):
+    """F_AUX of a fresh handle with the push schedule of each env's case (push count, the force of an EPMC push inside its window,
+    the draw index); every other case starts far before its push window"""
+    aux = eng.get(capi.F_AUX).copy()
+    rng = np.random.default_rng(rng_seed)
+    for i, c in enumerate(cases):
+        aux[i, capi.AUX_PUSH_COUNT] = {"push_in": 5 + (i // 2) % 7, "push_redraw": PUSH_INTERVAL - 1, "push_after": PUSH_DURATION - 1}.get(c, -1000)
+        h, th, v = rng.uniform(PUSH_MIN, 50.0), rng.uniform(-np.pi, np.pi), rng.uniform(0.0, 10.0)
+        aux[i, capi.AUX_PUSH_F:capi.AUX_PUSH_F + 3] = (h * np.cos(th), h * np.sin(th), v)
+        aux[i, capi.AUX_PUSH_DRAWS] = 1 + 2 * (i // 2)
+    return aux
+
+
+PUSH_INTERVAL, PUSH_DURATION = EPMC_CFG["push_interval_steps"], EPMC_CFG["push_duration_steps"]
+
+
+def dyn_run(oracle_lib, blob, mocap, kind, element, states, aux, acts, warm=None, **over):
+    """one oracle sub-step of the dynamics batch with pushes on; returns (state after, F_AUX after, warm start after)"""
+    n = len(states)
+    e = make(oracle_lib, kind, n, blob, mocap, element, **dict(dict(push_enabled=1), **over))
+    e.set(capi.F_STATE, states); e.set(capi.F_WARMSTART, np.zeros((n, 32), np.float32) if warm is None else warm); e.set(capi.F_AUX, aux)
+    e.step(acts)
+    out = (e.get(capi.F_STATE).astype(np.float64), e.get(capi.F_AUX).copy(), e.get(capi.F_WARMSTART).copy())
+    e.close()
+    return out
+
+
+def designed_dynamics(kind, oracle_lib, blob, mocap, element):
+    """dynamics_batch with its F_AUX: the draw index of every drawn push moved on until each force drawn is at least PUSH_MIN; in
+    the vel_clamp envs the four velocity entries inside the bound that change most in the sub-step are put half their change
+    (v' - v, measured on the oracle with max_coord_vel at 1e9) inside it, so that v + a dt crosses it, a few times over as a depends
+    on v.  Returns (states, decisions, F_AUX, actions, case per env, llq_config)."""
+    states, decs, acts, cases, cfg = dynamics_batch(kind, oracle_lib, blob, mocap, element)
+    n = len(states)
+    e = make(oracle_lib, kind, n, blob, mocap, element, push_enabled=1)
+    aux = push_aux(e, cases, SEED)
+    e.close()
+    vmax = cfg.max_coord_vel
+    vc = np.flatnonzero(np.array(cases) == "vel_clamp")
+    for _ in range(6):
+        after = dyn_run(oracle_lib, blob, mocap, kind, element, states, aux, acts, max_coord_vel=1e9)[0]
+        if (crossings(states[vc], after[vc], vmax)[0] > 0).all():
+            break
+        for i in vc:
+            v0 = states[i, VEL].astype(np.float64)
+            dv = after[i, VEL] - v0
+            cand = [j for j in np.argsort(-np.abs(dv)) if abs(v0[j]) <= vmax and abs(dv[j]) > 1e-2][:4]
+            for j in cand:
+                states[i, VEL[j]] = np.sign(dv[j]) * (vmax - 0.5 * abs(dv[j]))
+    else:
+        raise RuntimeError("no velocity the sub-step carries across the bound")
+    pushed = np.array([c.startswith("push") for c in cases])
+    for _ in range(50):
+        after = dyn_run(oracle_lib, blob, mocap, kind, element, states, aux, acts)[1]
+        f = np.linalg.norm(after[:, capi.AUX_PUSH_F:capi.AUX_PUSH_F + 3], axis=1)
+        weak = pushed & (f < PUSH_MIN)
+        if kind == "sepmc":
+            weak = np.repeat(weak.reshape(-1, 2).any(1), 2)
+        if not weak.any():
+            return states, decs, aux, acts, cases, cfg
+        aux[weak, capi.AUX_PUSH_DRAWS] += 2 * n
+    raise RuntimeError("no draw index gives pushes of PUSH_MIN")
+
+
+DYN_BAR = 2e-5            # TOL1 at solver_iters 1 / 10: the visibility checks ask for 100x this
+STATE_BLOCKS = {"pose": np.r_[0:7, 13:25], "base velocity": np.r_[7:13], "joint velocity": np.r_[25:37]}
+
+
+def blockwise(a, b):
+    """blockrel per state block (pose, base velocity, joint velocity): a 100 m/s velocity does not scale the pose comparison"""
+    from test_parity_gpu import blockrel
+    return {k: blockrel(a[:, ix], b[:, ix]) for k, ix in STATE_BLOCKS.items()}
+
+
+@pytest.mark.parametrize("kind,element", DYN_KINDS)
+def test_pushes_and_clamps_are_designed_and_visible(kind, element, oracle_lib, blob, small_mocap):
+    """Every env of the dynamics batch takes its designed branches on the oracle (as in the solver pin), reaches its category (the PD
+    clamps per joint; in every vel_clamp env an entry the sub-step carries across the bound and one beyond it) and is visible: the
+    same step with the push off, or with max_tau / max_coord_vel at 1e9, moves the post-step state by at least 100x the GPU bar in
+    some state block (a push after its window: not at all, and the same env one sub-step earlier in the window: by 100x)."""
+    states, decs, aux, acts, cases, cfg = designed_dynamics(kind, oracle_lib, blob, small_mocap, element)
+    cases = np.array(cases)
+    # every state takes its designed branches on the oracle (a pair of copies for SEPMC, the env's own corridor)
+    worst = oracle_one_by_one(oracle_lib, blob, small_mocap, kind, element, states, decs)
+    assert all(d["n_off_ground"] == 0 for d in decs)
+    for i in np.flatnonzero(cases == "pd_clamp"):
+        assert {"+target", "-target", "+tau", "-tau"} <= set(pd_categories(states[i], acts[i], cfg.kp, cfg.kd, cfg.max_tau)), i
+    ref, aux_after, _ = dyn_run(oracle_lib, blob, small_mocap, kind, element, states, aux, acts)
+    def moved(other):
+        return np.max(np.stack(list(blockwise(other, ref).values())), axis=0)
+    off = dyn_run(oracle_lib, blob, small_mocap, kind, element, states, aux, acts, push_enabled=0)[0]
+    inwin = aux.copy(); inwin[:, capi.AUX_PUSH_COUNT] = np.where(cases == "push_after", PUSH_DURATION - 2, aux[:, capi.AUX_PUSH_COUNT])
+    earlier = dyn_run(oracle_lib, blob, small_mocap, kind, element, states, inwin, acts)[0]
+    no_tau = dyn_run(oracle_lib, blob, small_mocap, kind, element, states, aux, acts, max_tau=1e9)[0]
+    no_vel = dyn_run(oracle_lib, blob, small_mocap, kind, element, states, aux, acts, max_coord_vel=1e9)[0]
+    vc = cases == "vel_clamp"
+    cross, beyond = crossings(states[vc], no_vel[vc], cfg.max_coord_vel)
+    assert (cross > 0).all() and (beyond > 0).all(), (cross, beyond)
+    f = np.linalg.norm(aux_after[:, capi.AUX_PUSH_F:capi.AUX_PUSH_F + 3], axis=1)
+    pushed = np.char.startswith(cases.astype(str), "push")
+    assert np.all(f[pushed] >= PUSH_MIN), f[pushed]
+    if kind == "sepmc":
+        assert np.all(aux_after[0::2, capi.AUX_PUSH_DRAWS] == aux_after[1::2, capi.AUX_PUSH_DRAWS])
+    vis = {}
+    for c, m in (("push_in", moved(off)), ("push_redraw", moved(off)), ("push_after", moved(earlier)),
+                 ("pd_clamp", moved(no_tau)), ("vel_clamp", moved(no_vel)), ("vel_impulse", moved(no_vel))):
+        sel = cases == c
+        vis[c] = float(m[sel].min())
+        assert np.all(m[sel] >= 100 * DYN_BAR), (c, np.flatnonzero(sel & (m < 100 * DYN_BAR)), m[sel])
+    assert np.array_equal(moved(off)[cases == "push_after"], np.zeros((cases == "push_after").sum()))
+    print("%s: %d envs, smallest oracle decision margin %.1e; velocity entries carried across / starting beyond the bound per "
+          "vel_clamp env >= %d / %d; smallest visibility per case (block-relative change): %s" % (
+              kind, len(cases), worst, cross.min(), beyond.min(), ", ".join("%s %.1e" % kv for kv in vis.items())))

@@ -20,6 +20,14 @@ Bars (block-relative state error, and per-sphere normal impulse error over max(1
     iters 0   measured 8.2e-06  -> 5e-5
     iters 1   measured 1.0e-04  -> 5e-4
     iters 10  measured 1.5e-04  -> 1e-3
+
+The same bars hold the extensions of the pin, unchanged.  Largest error over the bar that applies, at any of solver_iters 0 / 1 / 10,
+measured on an H100 80GB HBM3 (700 W power limit):
+  EPMC flat arena (element 0)                                           0.21
+  corridor element 2, the bars (bottom faces, corners inside, bottom-edge cylinders, ground and bar at once)   0.22
+  knee_contacts 0 (feet): PMC 0.20, SEPMC 0.22, corridor element 1 0.24
+  knee_contacts 1 (feet, knee wheels, one contact per leg): PMC 0.19, SEPMC 0.46 (9.1e-6 at iters 10 on the ground), corridor 0.17
+  pushes and clamps, per state block: EPMC flat 0.17, SEPMC 0.24, corridor element 1 0.19
 """
 import numpy as np
 import pytest
@@ -27,7 +35,7 @@ import pytest
 import solver_cases as sc
 from lifelike_agility_and_play_b200 import _capi as capi
 from test_parity_gpu import blockrel
-from test_solver_cases import KINDS, designed_batch, make
+from test_solver_cases import DYN_KINDS, KINDS, LEGACY, blockwise, designed_batch, designed_dynamics, make
 
 pytestmark = pytest.mark.gpu
 
@@ -38,9 +46,11 @@ FIELDS = {"pmc": (capi.F_STATE, capi.F_WARMSTART, capi.F_OBS, capi.F_TIME, capi.
           "other": (capi.F_STATE, capi.F_WARMSTART, capi.F_OBS, capi.F_TIME, capi.F_AUX, capi.F_EPISODE_ID, capi.F_REWARD_SUM)}
 
 
-def one_step(gpu, cpu, kind, states, warm, actions):
+def one_step(gpu, cpu, kind, states, warm, actions, aux=None):
     """teacher-forced sub-step from the designed states; returns (state err per env, impulse err per env, counters gpu, cpu)"""
     cpu.set(capi.F_STATE, states); cpu.set(capi.F_WARMSTART, warm)
+    if aux is not None:
+        cpu.set(capi.F_AUX, aux)
     for f in FIELDS["pmc" if kind == "pmc" else "other"]:
         gpu.set(f, cpu.get(f))
     g0, c0 = gpu.counters().copy(), cpu.counters().copy()
@@ -54,35 +64,71 @@ def one_step(gpu, cpu, kind, states, warm, actions):
     return e, el, same_set, gpu.counters() - g0, cpu.counters() - c0
 
 
-@pytest.mark.parametrize("kind,element", KINDS)
-def test_designed_substeps_match_the_oracle_env_by_env(kind, element, built, blob, small_mocap, oracle_lib):
-    states, decs = designed_batch(kind, oracle_lib, blob, small_mocap, element)
+def compare(kind, element, states, decs, blob, small_mocap, oracle_lib, actions=None, aux=None, blocks=False, **over):
+    """every env of a designed batch, one sub-step on both engines at solver_iters 0 / 1 / 10, with and without a warm start: the
+    rows solved and dropped are equal, so is the set of spheres with a normal impulse, and the state (blocks: each state block on its
+    own) and the impulses are within the bars.  Returns the largest error per iteration count over the bar that applies."""
     n = len(states)
-    mapping, reached = sc.warp_cases([d["nc"] for d in decs], [d["nl"] for d in decs])
-    print("%s element %d: %d envs, mapping cases %s" % (kind, element, n, sorted(reached)))
-    assert reached & {"two_pass", "borrow", "contact_cap", "limit_cap"}, "the batch reaches none of the solver's heavy paths"
     rng = np.random.default_rng(7)
     warm_nz = rng.uniform(0.0, 3.0, (n, 32)).astype(np.float32)       # also on spheres without contact: both engines must drop it
-    actions = np.clip(0.3 * rng.standard_normal((n, 12)), -1, 1).astype(np.float32)
+    a = np.clip(0.3 * rng.standard_normal((n, 12)), -1, 1).astype(np.float32)
+    actions = a if actions is None else actions
     off_ground = np.array([d["n_off_ground"] > 0 for d in decs])      # a wall, box or edge-cylinder contact: TOL1_FP32_STATICS
     print("  %d of %d envs touch a wall, box or edge cylinder" % (off_ground.sum(), n))
+    ratio = {}
     for iters in (0, 1, 10):
         bar = np.where(off_ground, TOL1_FP32_STATICS[iters], TOL1[iters])
         worst = {True: 0.0, False: 0.0}
+        ratio[iters] = 0.0
         for warm in (np.zeros((n, 32), np.float32), warm_nz):
-            gpu = make(capi.load_cuda_library(), kind, n, blob, small_mocap, element, solver_iters=iters)
-            cpu = make(oracle_lib, kind, n, blob, small_mocap, element, solver_iters=iters)
-            e, el, same, cg, cc = one_step(gpu, cpu, kind, states, warm, actions)
+            gpu = make(capi.load_cuda_library(), kind, n, blob, small_mocap, element, solver_iters=iters, **over)
+            cpu = make(oracle_lib, kind, n, blob, small_mocap, element, solver_iters=iters, **over)
+            e, el, same, cg, cc = one_step(gpu, cpu, kind, states, warm, actions, aux)
+            if blocks:
+                per = blockwise(gpu.get(capi.F_STATE), cpu.get(capi.F_STATE))
+                e = np.max(np.stack(list(per.values())), axis=0)
             gpu.close(); cpu.close()
             for k in (True, False):
                 if (off_ground == k).any():
                     worst[k] = max(worst[k], np.maximum(e, el)[off_ground == k].max())
+            ratio[iters] = max(ratio[iters], float(np.max(np.maximum(e, el) / bar)))
             assert (cg[2], cg[3], cg[5]) == (cc[2], cc[3], cc[5]), ("rows solved / dropped", iters, cg[:6], cc[:6])
             assert same.all(), ("envs whose set of spheres with a normal impulse differs", np.flatnonzero(~same))
             assert np.all(e < bar), ("state", iters, np.flatnonzero(e >= bar), e.max())
             assert np.all(el < bar), ("impulse", iters, np.flatnonzero(el >= bar), el.max())
         print("  solver_iters %2d: max state / impulse err %.1e on the ground alone (bar %.0e), %.1e with a wall, box or cylinder (bar %.0e)" % (
             iters, worst[False], TOL1[iters], worst[True], TOL1_FP32_STATICS[iters]))
+    return ratio
+
+
+@pytest.mark.parametrize("kind,element", KINDS)
+def test_designed_substeps_match_the_oracle_env_by_env(kind, element, built, blob, small_mocap, oracle_lib):
+    states, decs = designed_batch(kind, oracle_lib, blob, small_mocap, element)
+    mapping, reached = sc.warp_cases([d["nc"] for d in decs], [d["nl"] for d in decs])
+    print("%s element %d: %d envs, mapping cases %s" % (kind, element, len(states), sorted(reached)))
+    assert reached & {"two_pass", "borrow", "contact_cap", "limit_cap"}, "the batch reaches none of the solver's heavy paths"
+    ratio = compare(kind, element, states, decs, blob, small_mocap, oracle_lib)
+    print("  largest error over its bar: %s" % ratio)
+
+
+@pytest.mark.parametrize("kind,element,rule", LEGACY)
+def test_legacy_contact_sets_match_the_oracle_env_by_env(kind, element, rule, built, blob, small_mocap, oracle_lib):
+    """knee_contacts 0 and 1: the feet alone, or feet and knee wheels with one contact per leg (the deeper one, in leg order)"""
+    states, decs = designed_batch(kind, oracle_lib, blob, small_mocap, element, rule)
+    print("%s element %d rule %d: %d envs, mapping cases %s" % (kind, element, rule, len(states),
+                                                              sorted(sc.warp_cases([d["nc"] for d in decs], [d["nl"] for d in decs])[1])))
+    ratio = compare(kind, element, states, decs, blob, small_mocap, oracle_lib, knee_contacts=rule)
+    print("  largest error over its bar: %s" % ratio)
+
+
+@pytest.mark.parametrize("kind,element", DYN_KINDS)
+def test_pushes_and_clamps_match_the_oracle_env_by_env(kind, element, built, blob, small_mocap, oracle_lib):
+    """pushes inside their window, on the first sub-step after a redraw and just after the window; the PD target and torque clamps;
+    velocities at the +-max_coord_vel bound before and after the impulses -- compared per state block"""
+    states, decs, aux, acts, cases, _ = designed_dynamics(kind, oracle_lib, blob, small_mocap, element)
+    print("%s element %d: %d envs" % (kind, element, len(states)))
+    ratio = compare(kind, element, states, decs, blob, small_mocap, oracle_lib, actions=acts, aux=aux, blocks=True, push_enabled=1)
+    print("  largest error over its bar: %s" % ratio)
 
 
 # ---------------------------------------------------------------------------------------------------------------- placement
