@@ -52,7 +52,8 @@ const char* llq_policy_last_error(void);
 /* ---- environmental- and strategic-level policies (csrc/llq_policy_hier.cu): conv encoders + layer-norm LSTMs + the frozen
  * primitive-level decoder, one CTA per observation row, fp32 on the CUDA cores.  Replaces `PGAgent.step(obs, argmax=True)` of
  * test_scripts/environmental_level/test_environmental_level_env.py:95-100 and test_scripts/strategic_level/test_strategic_level_env.py:96
- * (mean heading, argmax code, mean action) for a whole batch of envs; nets: networks/legged_robot/epmc_net/epmc_net.py:86-177,
+ * (mean heading, argmax code, mean action) for a whole batch of envs, and at the environmental level also the actor step of a
+ * training rollout (sampled code, -log p, V; llq_hier_policy_forward_rec); nets: networks/legged_robot/epmc_net/epmc_net.py:86-177,
  * networks/legged_robot/sepmc_net/sepmc_net.py:122-203, networks/legged_robot/pmc_net/pmc_net.py:99-112.
  * `weights`: all arrays of the shipped *.model file, fp32, concatenated; `offsets[role]`: start of the array that plays `role`
  * (the host-side table is lifelike_agility_and_play_b200/policy_epmc.py::hier_role_arrays):
@@ -62,9 +63,19 @@ const char* llq_policy_last_error(void);
  *   84-87 game-vector fc x 2, 88-89 embed, 90-98 LSTM, 99-100 heading fc. */
 #define LLQ_HIER_ROLES_MLC 56
 #define LLQ_HIER_ROLES_ALL 101
+/* The value tower of the environmental level, arrays 2-46 of environmental_level_*.model, as its own table (its 45 entries next to
+ * the 56 of the code controller would be indistinguishable from the strategic level's 101 by length):
+ *   0-1 prop fc W b (135 -> 128), 2-29 usr_cmd_encoder (as roles 4-31), 30-31 command fc (64 -> 128), 32-33 fc (256 -> 256),
+ *   34-42 LSTM (as roles 34-42), 43-44 value fc (32 -> 1, linear). */
+#define LLQ_HIER_ROLES_VALUE 45
 typedef struct llq_hier_policy* llq_hier_policy_handle;
 int llq_hier_policy_create(const float* weights, int64_t n_weights, const int32_t* offsets, int32_t n_roles, int32_t strategic, int32_t device,
                            llq_hier_policy_handle* out);
+/* Training handle of the environmental level (for llq_hier_policy_forward_rec): as llq_hier_policy_create with strategic = 0, plus
+ * `value_offsets[LLQ_HIER_ROLES_VALUE]` (n_value_roles must equal it).  strategic != 0 returns LLQ_EUNSUPPORTED: the strategic
+ * level's heading head is not built for training. */
+int llq_hier_policy_create_train(const float* weights, int64_t n_weights, const int32_t* offsets, int32_t n_roles, const int32_t* value_offsets,
+                                 int32_t n_value_roles, int32_t strategic, int32_t device, llq_hier_policy_handle* out);
 int llq_hier_policy_destroy(llq_hier_policy_handle h);
 /* d_actions[n,12] = mean action for d_obs[n, >= 916 (environmental) / 965 (strategic)] (device pointers, obs_ld = row stride in floats).
  * d_state [n, 64 / 128] floats: the LSTM states ([c, h] of the heading LSTM first at the strategic level), updated in place; rows whose
@@ -72,6 +83,19 @@ int llq_hier_policy_destroy(llq_hier_policy_handle h);
  * d_codes (int32[n]) / d_heading (float[n], strategic level) are optional outputs.  Asynchronous on `stream`. */
 int llq_hier_policy_forward(llq_hier_policy_handle h, const float* d_obs, int64_t obs_ld, int32_t n, const uint8_t* d_done, float* d_state,
                             float* d_actions, int32_t* d_codes, float* d_heading, void* stream);
+/* Actor step of a training rollout at the environmental level (agent.step(argmax=False)), on a handle from
+ * llq_hier_policy_create_train; llq_hier_policy_forward refuses such a handle.  As llq_hier_policy_forward, plus:
+ *   the code is SAMPLED from the 256-way head by Gumbel-max, code = argmax_j (logit_j - log(-log u_j)) (first index on ties), with
+ *     u = min((r + 1/2) 2^-32, 0.99999994f) in fp32 and r from Philox4x32-10, counter (low 32 bits of row_gid0 + i, q, `counter` lo,
+ *     `counter` hi), key (`seed` lo, `seed` hi), q = 0..63 giving the draws of logits 4q..4q+3 -- keyed by the GLOBAL row as in
+ *     llq_policy_forward_rec; pass a different `counter` every step.  d_actions is the decoder's action on the sampled code, and
+ *     d_codes (int32[n], nullable) receives the sampled code;
+ *   d_values[i * out_ld] (nullable): V of the value tower;  d_neglogp[i * out_ld] (nullable): -log p of the sampled code,
+ *     m + log sum_j exp(logit_j - m) - logit_code with m the largest logit;  out_ld = the slab's row stride puts both into a record row;
+ *   d_state [n, 128]: [c, h] of the code LSTM, then [c, h] of the value LSTM; both halves start from zero where d_done[i] != 0. */
+int llq_hier_policy_forward_rec(llq_hier_policy_handle h, const float* d_obs, int64_t obs_ld, int32_t n, const uint8_t* d_done, float* d_state,
+                                float* d_actions, int32_t* d_codes, float* d_values, float* d_neglogp, int64_t out_ld, uint64_t seed,
+                                uint64_t counter, int64_t row_gid0, void* stream);
 const char* llq_hier_policy_last_error(void);
 
 #ifdef __cplusplus

@@ -20,6 +20,7 @@
 #include <vector>
 #include "../../include/llq.h"
 #include "../../include/llq_policy.h"
+#include "llq_philox.cuh"
 
 #ifndef LLQ_POLICY_KU
 #define LLQ_POLICY_KU 4      // k-steps of weight fragments per register buffer (two buffers)
@@ -145,18 +146,6 @@ __device__ __forceinline__ void mma_layer(const float* A, int lda, Layer L, floa
         out[col * M + row + 8] = v2; out[(col + 1) * M + row + 8] = v3;
       }
     }
-}
-
-// Philox4x32-10 (same generator as the engine's reset streams, csrc/llq_math.cuh)
-__device__ __forceinline__ uint4 philox4x32(uint4 c, uint2 k) {
-#pragma unroll
-  for (int r = 0; r < 10; r++) {
-    const uint32_t h0 = __umulhi(0xD2511F53u, c.x), l0 = 0xD2511F53u * c.x;
-    const uint32_t h1 = __umulhi(0xCD9E8D57u, c.z), l1 = 0xCD9E8D57u * c.z;
-    c = make_uint4(h1 ^ c.y ^ k.x, l1, h0 ^ c.w ^ k.y, l0);
-    k.x += 0x9E3779B9u; k.y += 0xBB67AE85u;
-  }
-  return c;
 }
 
 __global__ void __launch_bounds__(THREADS) pmc_policy_kernel(const float* __restrict__ obs, long long ld, int n, Weights w,

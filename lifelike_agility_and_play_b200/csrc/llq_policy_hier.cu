@@ -9,6 +9,10 @@
 // The LSTM is `tpolicies`' layer-norm LSTM (absent from the reference tree), restated as in lifelike_agility_and_play_b200/policy_epmc.py,
 // which is the host statement of the same nets and the checker of this kernel (tests/test_policy_epmc.py).
 //
+// Training instance (environmental level only, llq_hier_policy_forward_rec): the value tower (arrays 2-46 of the shipped file), a
+// Gumbel-max sample of the 256-way code head with its -log p, and the decoder on the SAMPLED code; its recurrent state per row is
+// [c, h] of the code LSTM, then [c, h] of the value LSTM.
+//
 // One CTA (256 threads) per 8 observation rows; activations in shared memory (89 kB), weights (1.2 MB, fp32) streamed from L2 with
 // every thread of a layer reading consecutive columns and using each weight for all 8 rows; 0.23 M MAC per row on the CUDA cores.
 // The recurrent states live in device memory next to the engine's arrays and are wiped where the `done` flag of the previous
@@ -21,6 +25,7 @@
 
 #include "../../include/llq.h"
 #include "../../include/llq_policy.h"
+#include "llq_philox.cuh"
 
 namespace {
 
@@ -38,6 +43,12 @@ enum Role {
   R_N_ALL
 };
 static_assert(R_N_MLC == LLQ_HIER_ROLES_MLC && R_N_ALL == LLQ_HIER_ROLES_ALL, "role table (include/llq_policy.h)");
+// the value tower's table (arrays 2-46) follows the 101 roles above in the device offset table
+enum ValueRole {
+  V_PROP_W = 0, V_PROP_B, V_ENC /* 28 */, V_CMD_W = V_ENC + 28, V_CMD_B, V_FC3_W, V_FC3_B, V_LSTM /* 9 */, V_OUT_W = V_LSTM + 9, V_OUT_B, V_N
+};
+static_assert(V_N == LLQ_HIER_ROLES_VALUE, "value-tower table (include/llq_policy.h)");
+constexpr int RV = R_N_ALL;
 
 struct Net { const float* w; const int* off; };
 __device__ __forceinline__ const float* arr(const Net& n, int role) { return n.w + n.off[role]; }
@@ -248,12 +259,23 @@ struct alignas(16) Smem {
   int code[kRows], live[kRows], wipe[kRows];
 };
 
+// outputs and noise key of the training instance (unused by the deterministic one)
+struct Sample { float* values; float* neglogp; long long out_ld; unsigned long long seed, counter; long long row_gid0; };
+
+// g = -log(-log u) of one Philox word: u = (r + 1/2) 2^-32 in fp32, clamped below 1 (r >= 2^32 - 128 rounds to 1.0f, g would be +inf)
+__device__ __forceinline__ float gumbel(uint32_t r) {
+  const float u = fminf(((float)r + 0.5f) * 2.3283064365386963e-10f, 0.99999994f);
+  return -logf(-logf(u));
+}
+
+template <bool TRAIN>
 __global__ void __launch_bounds__(kThreads) hier_policy_kernel(Net net, int strategic, const float* __restrict__ obs, long long obs_ld, int n_rows,
                                                                const unsigned char* __restrict__ done, float* __restrict__ state, float* __restrict__ actions,
-                                                               int* __restrict__ codes, float* __restrict__ heading) {
+                                                               int* __restrict__ codes, float* __restrict__ heading, Sample smp) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   Smem& S = *reinterpret_cast<Smem*>(smem_raw);
   const int row0 = blockIdx.x * kRows, t = threadIdx.x;
+  if constexpr (TRAIN) strategic = 0;                       // the training instance serves the environmental level only
   const int ow = strategic ? 965 : 916;
   if (t < kRows) {
     const int live = row0 + t < n_rows;
@@ -270,7 +292,7 @@ __global__ void __launch_bounds__(kThreads) hier_policy_kernel(Net net, int stra
     S.p[r][i] = fminf(fmaxf((S.obs[r][i] - arr(net, R_MEAN)[i]) / (arr(net, R_STD)[i] + 1e-8f), -5.f), 5.f);
   }
   __syncthreads();
-  const int ssz = strategic ? 128 : 64;
+  const int ssz = (TRAIN || strategic) ? 128 : 64;
   float* st = state + (size_t)row0 * ssz;
   if (strategic) {
     // ---- heading controller
@@ -296,6 +318,28 @@ __global__ void __launch_bounds__(kThreads) hier_policy_kernel(Net net, int stra
     __syncthreads();
     st += 64;
   }
+  if constexpr (TRAIN) {
+    // ---- value tower (arrays 2-46), wired like the code controller: [prop 135 -> 128 | command encoder -> 64 -> 128] -> 256 -> LSTM(32)
+    // -> V (linear); its [c, h] is the second half of the row's state
+    dense(&S.p[0][0], 136, 135, arr(net, RV + V_PROP_W), arr(net, RV + V_PROP_B), 128, &S.cat[0][0], 256, S.scr, true);       // cat[0..128)
+    if (t < kRows * 3) {
+      const int r = t / 3, i = t - 3 * r;
+      S.y[r][i] = S.obs[r][913 + i];
+    }
+    __syncthreads();
+    dense(&S.y[0][0], 256, 3, arr(net, RV + V_ENC + 24), arr(net, RV + V_ENC + 25), 32, &S.x[0][0], 256, S.scr, true);       // x[0..32)
+    perception(net, RV + V_ENC, &S.obs[0][0], kObsLd, S.a, S.b, &S.x[0][32], 256);                                          // x[32..120)
+    dense(&S.x[0][0], 256, 120, arr(net, RV + V_ENC + 26), arr(net, RV + V_ENC + 27), 64, &S.y[0][0], 256, S.scr, true);     // y[0..64)
+    dense(&S.y[0][0], 256, 64, arr(net, RV + V_CMD_W), arr(net, RV + V_CMD_B), 128, &S.cat[0][128], 256, S.scr, true);       // cat[128..256)
+    dense(&S.cat[0][0], 256, 256, arr(net, RV + V_FC3_W), arr(net, RV + V_FC3_B), 256, &S.x[0][0], 256, S.scr, true);
+    lstm_step(net, RV + V_LSTM, &S.x[0][0], st + 64, ssz, S.live, S.wipe, &S.zx[0][0], &S.zh[0][0], &S.c[0][0], &S.h[0][0], S.scr);
+    if (t < kRows) {
+      float v = arr(net, RV + V_OUT_B)[0];
+      for (int k = 0; k < 32; k++) v = fmaf(S.h[t][k], arr(net, RV + V_OUT_W)[k], v);
+      if (smp.values && S.live[t]) smp.values[(size_t)(row0 + t) * smp.out_ld] = v;
+    }
+    __syncthreads();
+  }
   // ---- code controller (environmental level)
   dense(&S.p[0][0], 136, 135, arr(net, R_MPROP_W), arr(net, R_MPROP_B), 64, &S.cat[0][0], 256, S.scr, true);                // cat[0..64)
   if (t < kRows * 3) {
@@ -309,7 +353,39 @@ __global__ void __launch_bounds__(kThreads) hier_policy_kernel(Net net, int stra
   dense(&S.cat[0][0], 256, 128, arr(net, R_MEMB_W), arr(net, R_MEMB_B), 256, &S.x[0][0], 256, S.scr, true);
   lstm_step(net, R_MLSTM, &S.x[0][0], st, ssz, S.live, S.wipe, &S.zx[0][0], &S.zh[0][0], &S.c[0][0], &S.h[0][0], S.scr);
   dense(&S.h[0][0], 32, 32, arr(net, R_LOGIT_W), arr(net, R_LOGIT_B), 256, &S.y[0][0], 256, S.scr, false);                  // logits
-  {                                                         // argmax per row (warp r), first occurrence
+  if constexpr (TRAIN) {
+    // Gumbel-max sample: code = argmax_j (logit_j + g_j), g from Philox keyed (global row, q, counter) / seed, one call per four logits
+    for (int idx = t; idx < kRows * 64; idx += kThreads) {
+      const int r = idx >> 6, q = idx & 63;
+      const uint4 b = philox4x32(make_uint4((uint32_t)(smp.row_gid0 + row0 + r), (uint32_t)q, (uint32_t)smp.counter, (uint32_t)(smp.counter >> 32)),
+                                 make_uint2((uint32_t)smp.seed, (uint32_t)(smp.seed >> 32)));
+      *reinterpret_cast<float4*>(&S.x[r][4 * q]) = make_float4(gumbel(b.x), gumbel(b.y), gumbel(b.z), gumbel(b.w));
+    }
+    __syncthreads();
+    const int r = t >> 5, l = t & 31;
+    float best = -3.4e38f, m = -3.4e38f; int bi = 0;
+    for (int i = l; i < 256; i += 32) {
+      const float v = S.y[r][i] + S.x[r][i];
+      if (v > best) { best = v; bi = i; }
+      m = fmaxf(m, S.y[r][i]);
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+      const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+      if (ob > best || (ob == best && oi < bi)) { best = ob; bi = oi; }
+      m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    }
+    float se = 0.f;                                         // -log p = (m - l_code) + log sum exp(l_j - m): no overflow for large logits
+    for (int i = l; i < 256; i += 32) se += expf(S.y[r][i] - m);
+    for (int o = 16; o > 0; o >>= 1) se += __shfl_xor_sync(0xffffffffu, se, o);
+    if (l == 0) {
+      S.code[r] = bi;
+      if (S.live[r]) {
+        if (codes) codes[row0 + r] = bi;
+        if (smp.neglogp) smp.neglogp[(size_t)(row0 + r) * smp.out_ld] = (m - S.y[r][bi]) + logf(se);
+      }
+    }
+  } else {                                                  // argmax per row (warp r), first occurrence
     const int r = t >> 5, l = t & 31;
     float best = -3.4e38f; int bi = 0;
     for (int i = l; i < 256; i += 32) if (S.y[r][i] > best) { best = S.y[r][i]; bi = i; }
@@ -338,28 +414,33 @@ __global__ void __launch_bounds__(kThreads) hier_policy_kernel(Net net, int stra
 }  // namespace
 
 struct llq_hier_policy {
-  int device = 0, strategic = 0;
+  int device = 0, strategic = 0, train = 0;
   bool attr_set = false;
   float* d_w = nullptr;
   int* d_off = nullptr;
 };
 
-extern "C" {
+namespace {
 
-int llq_hier_policy_create(const float* weights, int64_t n_weights, const int32_t* offsets, int32_t n_roles, int32_t strategic, int32_t device,
-                           llq_hier_policy_handle* out) {
+// `value_offsets` (LLQ_HIER_ROLES_VALUE entries) null: a deterministic handle
+int create(const float* weights, int64_t n_weights, const int32_t* offsets, int32_t n_roles, const int32_t* value_offsets, int32_t strategic,
+           int32_t device, llq_hier_policy_handle* out) {
   if (!weights || !offsets || !out) return fail_h(LLQ_EINVAL, "null argument");
   if (n_roles != (strategic ? LLQ_HIER_ROLES_ALL : LLQ_HIER_ROLES_MLC)) return fail_h(LLQ_EINVAL, "role table has the wrong length (include/llq_policy.h)");
   for (int i = 0; i < n_roles; i++) if (offsets[i] < 0 || offsets[i] >= n_weights) return fail_h(LLQ_EINVAL, "role offset outside the weight blob");
+  if (value_offsets)
+    for (int i = 0; i < LLQ_HIER_ROLES_VALUE; i++)
+      if (value_offsets[i] < 0 || value_offsets[i] >= n_weights) return fail_h(LLQ_EINVAL, "value-tower offset outside the weight blob");
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail_h(LLQ_ECUDA, "no CUDA device visible (no CPU fallback)");
   if (device < 0 || device >= ndev) return fail_h(LLQ_EINVAL, "device ordinal out of range");
   if (cudaSetDevice(device) != cudaSuccess) return fail_h(LLQ_ECUDA, "cudaSetDevice failed");
   llq_hier_policy* h = new (std::nothrow) llq_hier_policy();
   if (!h) return fail_h(LLQ_ENOMEM, "out of memory");
-  h->device = device; h->strategic = strategic ? 1 : 0;
-  std::vector<int> off(LLQ_HIER_ROLES_ALL, 0);
+  h->device = device; h->strategic = strategic ? 1 : 0; h->train = value_offsets ? 1 : 0;
+  std::vector<int> off(RV + V_N, 0);
   for (int i = 0; i < n_roles; i++) off[i] = offsets[i];
+  if (value_offsets) for (int i = 0; i < V_N; i++) off[RV + i] = value_offsets[i];
   if (cudaMalloc(&h->d_w, sizeof(float) * (size_t)n_weights) != cudaSuccess || cudaMalloc(&h->d_off, sizeof(int) * off.size()) != cudaSuccess ||
       cudaMemcpy(h->d_w, weights, sizeof(float) * (size_t)n_weights, cudaMemcpyHostToDevice) != cudaSuccess ||
       cudaMemcpy(h->d_off, off.data(), sizeof(int) * off.size(), cudaMemcpyHostToDevice) != cudaSuccess) {
@@ -368,6 +449,40 @@ int llq_hier_policy_create(const float* weights, int64_t n_weights, const int32_
   }
   *out = h;
   return LLQ_OK;
+}
+
+template <bool TRAIN>
+int launch(llq_hier_policy_handle h, const float* d_obs, int64_t obs_ld, int32_t n, const uint8_t* d_done, float* d_state, float* d_actions,
+           int32_t* d_codes, float* d_heading, const Sample& smp, void* stream) {
+  if (cudaSetDevice(h->device) != cudaSuccess) return fail_h(LLQ_ECUDA, "cudaSetDevice failed");
+  Net net{h->d_w, h->d_off};
+  if (!h->attr_set) {
+    if (cudaFuncSetAttribute(hier_policy_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem)) != cudaSuccess ||
+        (h->train && cudaFuncSetAttribute(hier_policy_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem)) != cudaSuccess))
+      return fail_h(LLQ_ECUDA, "cudaFuncSetAttribute failed");
+    h->attr_set = true;                                      // per handle = per device
+  }
+  hier_policy_kernel<TRAIN><<<(n + kRows - 1) / kRows, kThreads, sizeof(Smem), (cudaStream_t)stream>>>(net, h->strategic, d_obs, obs_ld, n, d_done, d_state,
+                                                                                                    d_actions, d_codes, d_heading, smp);
+  if (cudaGetLastError() != cudaSuccess) return fail_h(LLQ_ECUDA, "hier_policy_kernel launch failed");
+  return LLQ_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int llq_hier_policy_create(const float* weights, int64_t n_weights, const int32_t* offsets, int32_t n_roles, int32_t strategic, int32_t device,
+                           llq_hier_policy_handle* out) {
+  return create(weights, n_weights, offsets, n_roles, nullptr, strategic, device, out);
+}
+
+int llq_hier_policy_create_train(const float* weights, int64_t n_weights, const int32_t* offsets, int32_t n_roles, const int32_t* value_offsets,
+                                 int32_t n_value_roles, int32_t strategic, int32_t device, llq_hier_policy_handle* out) {
+  if (strategic) return fail_h(LLQ_EUNSUPPORTED, "training rollouts exist for the environmental level only (include/llq_policy.h)");
+  if (!value_offsets) return fail_h(LLQ_EINVAL, "null argument");
+  if (n_value_roles != LLQ_HIER_ROLES_VALUE) return fail_h(LLQ_EINVAL, "value-tower table has the wrong length (include/llq_policy.h)");
+  return create(weights, n_weights, offsets, n_roles, value_offsets, 0, device, out);
 }
 
 int llq_hier_policy_destroy(llq_hier_policy_handle h) {
@@ -381,18 +496,19 @@ int llq_hier_policy_destroy(llq_hier_policy_handle h) {
 int llq_hier_policy_forward(llq_hier_policy_handle h, const float* d_obs, int64_t obs_ld, int32_t n, const uint8_t* d_done, float* d_state,
                             float* d_actions, int32_t* d_codes, float* d_heading, void* stream) {
   if (!h || !d_obs || !d_state || !d_actions) return fail_h(LLQ_EINVAL, "null argument");
+  if (h->train) return fail_h(LLQ_EINVAL, "a training handle steps with llq_hier_policy_forward_rec (its state rows are 128 floats)");
   if (n <= 0 || obs_ld < (h->strategic ? 965 : 916)) return fail_h(LLQ_EINVAL, "bad row count or row stride");
-  if (cudaSetDevice(h->device) != cudaSuccess) return fail_h(LLQ_ECUDA, "cudaSetDevice failed");
-  Net net{h->d_w, h->d_off};
-  if (!h->attr_set) {
-    if (cudaFuncSetAttribute(hier_policy_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem)) != cudaSuccess)
-      return fail_h(LLQ_ECUDA, "cudaFuncSetAttribute failed");
-    h->attr_set = true;                                      // per handle = per device
-  }
-  hier_policy_kernel<<<(n + kRows - 1) / kRows, kThreads, sizeof(Smem), (cudaStream_t)stream>>>(net, h->strategic, d_obs, obs_ld, n, d_done, d_state,
-                                                                                              d_actions, d_codes, d_heading);
-  if (cudaGetLastError() != cudaSuccess) return fail_h(LLQ_ECUDA, "hier_policy_kernel launch failed");
-  return LLQ_OK;
+  return launch<false>(h, d_obs, obs_ld, n, d_done, d_state, d_actions, d_codes, d_heading, Sample{}, stream);
+}
+
+int llq_hier_policy_forward_rec(llq_hier_policy_handle h, const float* d_obs, int64_t obs_ld, int32_t n, const uint8_t* d_done, float* d_state,
+                                float* d_actions, int32_t* d_codes, float* d_values, float* d_neglogp, int64_t out_ld, uint64_t seed, uint64_t counter,
+                                int64_t row_gid0, void* stream) {
+  if (!h || !d_obs || !d_state || !d_actions) return fail_h(LLQ_EINVAL, "null argument");
+  if (!h->train) return fail_h(LLQ_EINVAL, "not a training handle (llq_hier_policy_create_train)");
+  if (n <= 0 || obs_ld < 916 || out_ld < 1) return fail_h(LLQ_EINVAL, "bad row count or row stride");
+  const Sample smp{d_values, d_neglogp, (long long)out_ld, (unsigned long long)seed, (unsigned long long)counter, (long long)row_gid0};
+  return launch<true>(h, d_obs, obs_ld, n, d_done, d_state, d_actions, d_codes, nullptr, smp, stream);
 }
 
 const char* llq_hier_policy_last_error(void) { return g_err_h.c_str(); }

@@ -16,6 +16,11 @@ import torch.distributed as dist
 OBS_DIM, ACT_DIM = 207, 12
 COL_ACTION, COL_REWARD, COL_DONE, COL_NEGLOGP, COL_VALUE = 207, 219, 220, 221, 222
 TRAJ_WIDTH = 223
+# the environmental level's record (parallel/hier_rollout.py): obs 916 | action 12 | reward | done (the step kernel, record option 2) |
+# -log p | value | sampled code (as a float), padded to a multiple of 4 floats
+HIER_OBS_DIM = 916
+HCOL_ACTION, HCOL_REWARD, HCOL_DONE, HCOL_NEGLOGP, HCOL_VALUE, HCOL_CODE = 916, 928, 929, 930, 931, 932
+HIER_TRAJ_WIDTH = 936
 
 
 def shard_offset(rank, envs_per_rank):

@@ -25,7 +25,8 @@ from collections import OrderedDict
 import numpy as np
 import torch
 
-from .trajectory import ACT_DIM, COL_ACTION, COL_DONE, COL_NEGLOGP, COL_REWARD, COL_VALUE, OBS_DIM, TRAJ_WIDTH
+from .trajectory import (ACT_DIM, COL_ACTION, COL_DONE, COL_NEGLOGP, COL_REWARD, COL_VALUE, HCOL_CODE, HCOL_DONE, HCOL_NEGLOGP, HCOL_REWARD,
+                         HCOL_VALUE, HIER_TRAJ_WIDTH, OBS_DIM, TRAJ_WIDTH)
 
 OBS_LEAVES = OrderedDict([("prop", 99), ("prop_a", 36), ("future", 72)])        # PLE:117-124
 # leaf order of a flattened PMCInputs record (namedtuple order, the observation dict in key-insertion order)
@@ -70,6 +71,41 @@ def slab_records(slab, bootstrap_value=None, gamma=GAMMA, lam=LAM, flatparam=Non
     else:
         rec[:, :, c + 5:] = flatparam.transpose(0, 1)
     return rec
+
+
+# observation leaves of the environmental level (PGE:129-137), in the order of its 916 observation columns
+HIER_OBS_LEAVES = OrderedDict([("prop", (99,)), ("prop_a", (36,)), ("percep_2d", (25, 13)), ("percep_1d", (128,)), ("percep_front", (25, 13)),
+                               ("target", (3,))])
+
+
+def hier_slab_records(slab, initial_state, first_mask, bootstrap_value, gamma=GAMMA, lam=LAM):
+    """Learner tensors of an environmental-level unroll (`HierRolloutWorker.finish_unroll()`), on the slab's device, named:
+    the observation leaves [T, N, *leaf], `A_Z` [T, N] int64 (the sampled code), `neglogp`, `discount` = gamma (1 - done), `r`,
+    `V`, `R` (lambda-returns, bootstrapped with V(observation T)), `M` [T, N] = the mask each forward received (M[0] = first_mask,
+    M[t] = done[t-1]) -- all [T, N] float32 -- and `S` [N, 128], the recurrent state the unroll started from (code LSTM [c, h], then
+    value LSTM [c, h])."""
+    assert slab.dim() == 3 and slab.shape[2] == HIER_TRAJ_WIDTH, "expected a [T, N, %d] trajectory slab" % HIER_TRAJ_WIDTH
+    T, N, _ = slab.shape
+    out = OrderedDict()
+    c = 0
+    for name, shape in HIER_OBS_LEAVES.items():
+        k = int(np.prod(shape))
+        out[name] = slab[:, :, c:c + k].reshape(T, N, *shape)
+        c += k
+    r, done, v = slab[:, :, HCOL_REWARD], slab[:, :, HCOL_DONE], slab[:, :, HCOL_VALUE]
+    discount = gamma * (1.0 - done)
+    out["A_Z"] = slab[:, :, HCOL_CODE].to(torch.int64)
+    out["neglogp"] = slab[:, :, HCOL_NEGLOGP]
+    out["discount"] = discount
+    out["r"] = r
+    out["V"] = v
+    out["R"] = lambda_returns(r, discount, v, bootstrap_value.to(slab.dtype), lam)
+    mask = torch.empty((T, N), dtype=slab.dtype, device=slab.device)
+    mask[0] = (first_mask != 0).to(slab.dtype)
+    mask[1:] = (done[:-1] != 0).to(slab.dtype)
+    out["M"] = mask
+    out["S"] = initial_state
+    return out
 
 
 def slab_to_unrolls(slab, model_key, infos=None, **kw):

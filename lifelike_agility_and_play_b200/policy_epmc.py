@@ -155,10 +155,39 @@ class EpmcPolicy:
         o = np.asarray(obs, np.float32)
         return (o[:, 0:135], o[:, 135:460].reshape(-1, 25, 13), o[:, 460:588], o[:, 588:913].reshape(-1, 25, 13), o[:, 913:916])
 
-    def act(self, obs, state, mask, rng=None, return_code=False):
+    def value(self, obs, state, mask):
+        """V(obs) of the value tower (arrays 2-46), state [N, 64] = [c, h] of its own LSTM, mask as in `act`.  Returns (V [N], new state).
+
+        The wiring is restated from the array shapes with the code controller's conventions (the actor's value head of
+        example_epmc_train.sh; epmc_net.py's value part is not in the reference tree):
+            v1 = relu(p W2 + b3)                       135 -> 128   (p = the normalised, clipped prop)
+            ce = usr_cmd_encoder(arrays 4-31)          target 3 -> 32 | 3 perception encoders 88 -> 120 -> 64
+            v2 = relu(ce W32 + b33)                    64 -> 128
+            v3 = relu([v1 | v2] W34 + b35)             256 -> 256   (the code controller's [prop | command] order)
+            (c, h) = layer-norm LSTM(arrays 36-44)     state [c, h], zeroed where mask is set
+            V  = h W45 + b46                           32 -> 1, linear
+        Like the LSTM restatement above, nothing pins this against TensorFlow here: there is no TF, no shipped model file and no
+        epmc_net.py value code in this tree.  It is the statement the device's training forward (llq_hier_policy_forward_rec) is
+        checked against."""
+        prop, p2d, p1d, pfr, tgt = self.split(obs)
+        p = np.clip((prop - self.mean) / (self.std + 1e-8), -5.0, 5.0)
+        v1 = np.maximum(p @ self.vf_fc1[0] + self.vf_fc1[1], 0.0)
+        v2 = np.maximum(self.vf_cmd(p2d, p1d, pfr, tgt) @ self.vf_fc2[0] + self.vf_fc2[1], 0.0)
+        v3 = np.maximum(np.concatenate([v1, v2], axis=1) @ self.vf_fc3[0] + self.vf_fc3[1], 0.0)
+        h, state = self.vf_lstm.step(v3, state, np.asarray(mask, np.float32))
+        return (h @ self.vf_out[0] + self.vf_out[1])[:, 0].astype(np.float32), state
+
+    @staticmethod
+    def gumbel(uniforms):
+        """g = -log(-log u) of the Gumbel-max sample (fp64)."""
+        return -np.log(-np.log(np.asarray(uniforms, np.float64)))
+
+    def act(self, obs, state, mask, rng=None, return_code=False, uniforms=None, return_neglogp=False):
         """obs [N, 916] (prop 99 | prop_a 36 | percep_2d 325 | percep_1d 128 | percep_front 325 | target 3), state [N, 64] of the z-LSTM,
         mask [N] = 1 where the observation is the first of an episode.  `rng`: sample the code from the logits (the actor's
-        behaviour) instead of the argmax.  Returns (action [N, 12], new state)."""
+        behaviour) instead of the argmax; `uniforms` [N, 256] in (0, 1): sample it from these draws, code = argmax(logits + gumbel(u))
+        (the device's training forward draws them from Philox, include/llq_policy.h).  Returns (action [N, 12], new state), then the
+        code with `return_code`, then -log p of the code under the 256-way categorical with `return_neglogp`."""
         prop, p2d, p1d, pfr, tgt = self.split(obs)
         p = np.clip((prop - self.mean) / (self.std + 1e-8), -5.0, 5.0)
         pe = np.maximum(p @ self.prop_embed[0] + self.prop_embed[1], 0.0)
@@ -166,7 +195,9 @@ class EpmcPolicy:
         e = np.maximum(np.concatenate([pe, ce], axis=1) @ self.embed[0] + self.embed[1], 0.0)
         h, state = self.lstm.step(e, state, np.asarray(mask, np.float32))
         logits = h @ self.logits[0] + self.logits[1]
-        if rng is None:
+        if uniforms is not None:
+            code = (logits + self.gumbel(uniforms)).argmax(1)
+        elif rng is None:
             code = logits.argmax(1)
         else:
             g = -np.log(-np.log(rng.uniform(1e-12, 1.0, logits.shape)))
@@ -178,7 +209,12 @@ class EpmcPolicy:
         x = np.maximum(x @ self.dec[0][0] + self.dec[0][1], 0.0)
         x = np.maximum(x @ self.dec[1][0] + self.dec[1][1], 0.0)
         act = (x @ self.dec[2][0] + self.dec[2][1]).astype(np.float32)
-        return (act, state, code) if return_code else (act, state)
+        out = (act, state) + ((code,) if return_code else ())
+        if return_neglogp:
+            lg = logits.astype(np.float64)
+            m = lg.max(1)
+            out += ((m - lg[np.arange(len(code)), code]) + np.log(np.exp(lg - m[:, None]).sum(1)),)
+        return out
 
 
 class SepmcPolicy:
@@ -255,8 +291,13 @@ def random_weights(strategic=False, seed=0):
 
 
 # ---------------------------------------------------------------------------------------------------------------- device side
-def hier_role_arrays(strategic):
-    """Index (in the shipped file's array list) of the array that plays each role of include/llq_policy.h."""
+def hier_role_arrays(strategic, value_tower=False):
+    """Index (in the shipped file's array list) of the array that plays each role of include/llq_policy.h; `value_tower`: the
+    environmental level's value-tower table (LLQ_HIER_ROLES_VALUE entries) instead."""
+    if value_tower:
+        if strategic:
+            raise ValueError("the value-tower table exists for the environmental level only")
+        return list(range(2, 47))
     if not strategic:
         return [0, 1, 47, 48] + list(range(49, 77)) + [77, 78] + list(range(79, 88)) + [88, 89, 90] + list(range(91, 101))
     mlc = [0, 1, 97, 98] + list(range(99, 127)) + [127, 128] + list(range(129, 138)) + [138, 139, 140] + list(range(141, 151))
@@ -266,9 +307,11 @@ def hier_role_arrays(strategic):
 
 class DeviceHierPolicy:
     """The environmental- / strategic-level policy on the GPU (csrc/llq_policy_hier.cu through include/llq_policy.h): reads the engine's
-    observation rows in place, keeps the LSTM states on the device, writes the actions the fused env step consumes."""
+    observation rows in place, keeps the LSTM states on the device, writes the actions the fused env step consumes.
+    `train=True` (environmental level only): the training handle, stepped with `forward_rec` (sampled code, -log p, V; state rows of
+    128 floats = code LSTM, then value LSTM)."""
 
-    def __init__(self, weights, device=0):
+    def __init__(self, weights, device=0, train=False):
         import ctypes as C
         from .policy import POLICY_LIB_PATH
         import os
@@ -284,12 +327,19 @@ class DeviceHierPolicy:
         off = np.array([starts[i] for i in hier_role_arrays(self.strategic)], np.int32)
         self.lib.llq_hier_policy_last_error.restype = C.c_char_p
         h = C.c_void_p()
-        rc = self.lib.llq_hier_policy_create(blob.ctypes.data_as(C.c_void_p), C.c_int64(blob.size), off.ctypes.data_as(C.c_void_p), C.c_int32(off.size),
-                                             C.c_int32(int(self.strategic)), C.c_int32(device), C.byref(h))
+        self.train = bool(train)
+        if self.train:
+            voff = np.array([starts[i] for i in hier_role_arrays(False, value_tower=True)], np.int32)      # a strategic handle is refused
+            rc = self.lib.llq_hier_policy_create_train(blob.ctypes.data_as(C.c_void_p), C.c_int64(blob.size), off.ctypes.data_as(C.c_void_p),
+                                                       C.c_int32(off.size), voff.ctypes.data_as(C.c_void_p), C.c_int32(voff.size),
+                                                       C.c_int32(int(self.strategic)), C.c_int32(device), C.byref(h))
+        else:
+            rc = self.lib.llq_hier_policy_create(blob.ctypes.data_as(C.c_void_p), C.c_int64(blob.size), off.ctypes.data_as(C.c_void_p),
+                                                 C.c_int32(off.size), C.c_int32(int(self.strategic)), C.c_int32(device), C.byref(h))
         if rc:
-            raise RuntimeError("llq_hier_policy_create: %s" % self.lib.llq_hier_policy_last_error().decode())
+            raise RuntimeError("llq_hier_policy_create%s: %s" % ("_train" if self.train else "", self.lib.llq_hier_policy_last_error().decode()))
         self._h = h
-        self.state_dim = 128 if self.strategic else 64
+        self.state_dim = 128 if (self.strategic or self.train) else 64
         self.obs_dim = 965 if self.strategic else 916
 
     def forward(self, obs_ptr, obs_ld, n, done_ptr, state_ptr, act_ptr, codes_ptr=None, heading_ptr=None, stream=None):
@@ -298,6 +348,18 @@ class DeviceHierPolicy:
                                               C.c_void_p(act_ptr), C.c_void_p(codes_ptr or 0), C.c_void_p(heading_ptr or 0), C.c_void_p(stream or 0))
         if rc:
             raise RuntimeError("llq_hier_policy_forward: %s" % self.lib.llq_hier_policy_last_error().decode())
+
+    def forward_rec(self, obs_ptr, obs_ld, n, done_ptr, state_ptr, act_ptr, codes_ptr, values_ptr, neglogp_ptr, out_ld, seed, counter, row_gid0=0,
+                    stream=None):
+        """Training step (include/llq_policy.h, llq_hier_policy_forward_rec): sampled code -> codes_ptr (int32), V / -log p of row i ->
+        values_ptr / neglogp_ptr + i * out_ld floats; the Gumbel noise is keyed by (row_gid0 + i, counter) and `seed`."""
+        C = self._C
+        rc = self.lib.llq_hier_policy_forward_rec(self._h, C.c_void_p(obs_ptr), C.c_int64(obs_ld), C.c_int32(n), C.c_void_p(done_ptr or 0),
+                                                  C.c_void_p(state_ptr), C.c_void_p(act_ptr), C.c_void_p(codes_ptr or 0), C.c_void_p(values_ptr or 0),
+                                                  C.c_void_p(neglogp_ptr or 0), C.c_int64(out_ld), C.c_uint64(seed), C.c_uint64(counter),
+                                                  C.c_int64(row_gid0), C.c_void_p(stream or 0))
+        if rc:
+            raise RuntimeError("llq_hier_policy_forward_rec: %s" % self.lib.llq_hier_policy_last_error().decode())
 
     def close(self):
         if self._h:
