@@ -52,8 +52,9 @@ const char* llq_policy_last_error(void);
 /* ---- environmental- and strategic-level policies (csrc/llq_policy_hier.cu): conv encoders + layer-norm LSTMs + the frozen
  * primitive-level decoder, one CTA per observation row, fp32 on the CUDA cores.  Replaces `PGAgent.step(obs, argmax=True)` of
  * test_scripts/environmental_level/test_environmental_level_env.py:95-100 and test_scripts/strategic_level/test_strategic_level_env.py:96
- * (mean heading, argmax code, mean action) for a whole batch of envs, and at the environmental level also the actor step of a
- * training rollout (sampled code, -log p, V; llq_hier_policy_forward_rec); nets: networks/legged_robot/epmc_net/epmc_net.py:86-177,
+ * (mean heading, argmax code, mean action) for a whole batch of envs, and at both levels also the actor step of a training rollout
+ * (environmental: sampled code, -log p, V, llq_hier_policy_forward_rec; strategic: sampled heading, -log p, V,
+ * llq_hier_policy_forward_rec_strategic); nets: networks/legged_robot/epmc_net/epmc_net.py:86-177,
  * networks/legged_robot/sepmc_net/sepmc_net.py:122-203, networks/legged_robot/pmc_net/pmc_net.py:99-112.
  * `weights`: all arrays of the shipped *.model file, fp32, concatenated; `offsets[role]`: start of the array that plays `role`
  * (the host-side table is lifelike_agility_and_play_b200/policy_epmc.py::hier_role_arrays):
@@ -68,14 +69,26 @@ const char* llq_policy_last_error(void);
  *   0-1 prop fc W b (135 -> 128), 2-29 usr_cmd_encoder (as roles 4-31), 30-31 command fc (64 -> 128), 32-33 fc (256 -> 256),
  *   34-42 LSTM (as roles 34-42), 43-44 value fc (32 -> 1, linear). */
 #define LLQ_HIER_ROLES_VALUE 45
+/* The strategic level's training table: its value tower, arrays 2-50 of strategic_level.model, then the heading logstd (array 96, (1, 1),
+ * the one Gaussian parameter of the heading-controller block 51-96):
+ *   0-1 prop fc W b (135 -> 128), 2-25 perception encoders (2-D map 8, lidar 8, front map 8; as roles 58-81), 26-27 perception fusion
+ *   fc (88 -> 64), 28-29 perception fc (64 -> 128), 30-35 game-vector fc x 3 (29 -> 64 -> 64 -> 128), 36-37 concatenation fc (384 -> 256,
+ *   input [prop | perception | game] as the heading controller's), 38-46 LSTM (as roles 34-42), 47-48 value fc (32 -> 1, linear),
+ *   49 heading logstd.  All fully connected layers but the last take a ReLU. */
+#define LLQ_HIER_ROLES_TRAIN_STRATEGIC 50
 typedef struct llq_hier_policy* llq_hier_policy_handle;
 int llq_hier_policy_create(const float* weights, int64_t n_weights, const int32_t* offsets, int32_t n_roles, int32_t strategic, int32_t device,
                            llq_hier_policy_handle* out);
 /* Training handle of the environmental level (for llq_hier_policy_forward_rec): as llq_hier_policy_create with strategic = 0, plus
- * `value_offsets[LLQ_HIER_ROLES_VALUE]` (n_value_roles must equal it).  strategic != 0 returns LLQ_EUNSUPPORTED: the strategic
- * level's heading head is not built for training. */
+ * `value_offsets[LLQ_HIER_ROLES_VALUE]` (n_value_roles must equal it).  strategic != 0 returns LLQ_EUNSUPPORTED: the strategic level's
+ * training handle comes from llq_hier_policy_create_train_strategic. */
 int llq_hier_policy_create_train(const float* weights, int64_t n_weights, const int32_t* offsets, int32_t n_roles, const int32_t* value_offsets,
                                  int32_t n_value_roles, int32_t strategic, int32_t device, llq_hier_policy_handle* out);
+/* Training handle of the strategic level (for llq_hier_policy_forward_rec_strategic): `offsets` is the 101-role table of
+ * llq_hier_policy_create at the strategic level, `train_offsets[LLQ_HIER_ROLES_TRAIN_STRATEGIC]` the table above (n_train_roles must
+ * equal it). */
+int llq_hier_policy_create_train_strategic(const float* weights, int64_t n_weights, const int32_t* offsets, int32_t n_roles,
+                                           const int32_t* train_offsets, int32_t n_train_roles, int32_t device, llq_hier_policy_handle* out);
 int llq_hier_policy_destroy(llq_hier_policy_handle h);
 /* d_actions[n,12] = mean action for d_obs[n, >= 916 (environmental) / 965 (strategic)] (device pointers, obs_ld = row stride in floats).
  * d_state [n, 64 / 128] floats: the LSTM states ([c, h] of the heading LSTM first at the strategic level), updated in place; rows whose
@@ -96,6 +109,20 @@ int llq_hier_policy_forward(llq_hier_policy_handle h, const float* d_obs, int64_
 int llq_hier_policy_forward_rec(llq_hier_policy_handle h, const float* d_obs, int64_t obs_ld, int32_t n, const uint8_t* d_done, float* d_state,
                                 float* d_actions, int32_t* d_codes, float* d_values, float* d_neglogp, int64_t out_ld, uint64_t seed,
                                 uint64_t counter, int64_t row_gid0, void* stream);
+/* Actor step of a training rollout at the strategic level, on a handle from llq_hier_policy_create_train_strategic (the other entries
+ * refuse such a handle, this one refuses every other handle and obs_ld < 965).  The heading is the level's action:
+ *   a = mu + exp(logstd) eps, eps = sqrt(-2 log u0) cos(2 pi u1) with u0 = min((r.x + 1/2) 2^-32, 0.99999994f) and u1 = r.y 2^-32 in fp32,
+ *     r from Philox4x32-10 with counter (low 32 bits of row_gid0 + i, 64, `counter` lo, `counter` hi) and key (`seed` lo, `seed` hi)
+ *     (q = 64: apart from the Gumbel draws q = 0..63 of llq_hier_policy_forward_rec); pass a different `counter` every step;
+ *   d_heading[i * out_ld] (nullable): the RAW a;  d_neglogp[i * out_ld] (nullable): its -log p = 0.5 eps^2 + logstd + 0.5 log(2 pi), fp32;
+ *   d_values[i * out_ld] (nullable): V of the strategic value tower;
+ *   the frozen code controller receives clip(a, +-3.14159265f), as in llq_hier_policy_forward, and takes the ARGMAX code (d_codes, int32[n],
+ *     nullable); d_actions [n, 12] (contiguous) is the decoder's mean action on that code;
+ *   d_state [n, 192]: [c, h] of the heading LSTM, of the code LSTM, then of the value LSTM; all three start from zero where d_done[i] != 0
+ *     (d_done nullable). */
+int llq_hier_policy_forward_rec_strategic(llq_hier_policy_handle h, const float* d_obs, int64_t obs_ld, int32_t n, const uint8_t* d_done,
+                                          float* d_state, float* d_actions, int32_t* d_codes, float* d_heading, float* d_values, float* d_neglogp,
+                                          int64_t out_ld, uint64_t seed, uint64_t counter, int64_t row_gid0, void* stream);
 const char* llq_hier_policy_last_error(void);
 
 #ifdef __cplusplus

@@ -9,9 +9,12 @@
 // The LSTM is `tpolicies`' layer-norm LSTM (absent from the reference tree), restated as in lifelike_agility_and_play_b200/policy_epmc.py,
 // which is the host statement of the same nets and the checker of this kernel (tests/test_policy_epmc.py).
 //
-// Training instance (environmental level only, llq_hier_policy_forward_rec): the value tower (arrays 2-46 of the shipped file), a
+// Training instance of the environmental level (llq_hier_policy_forward_rec): the value tower (arrays 2-46 of the shipped file), a
 // Gumbel-max sample of the 256-way code head with its -log p, and the decoder on the SAMPLED code; its recurrent state per row is
 // [c, h] of the code LSTM, then [c, h] of the value LSTM.
+// Training instance of the strategic level (llq_hier_policy_forward_rec_strategic): the heading SAMPLED from its Gaussian head
+// (mean + exp(logstd) eps, Box-Muller from Philox) with its -log p, the clipped sample feeding the frozen code controller (argmax code)
+// and decoder, and the value tower of the strategic file (arrays 2-50); state per row: heading LSTM, code LSTM, value LSTM ([c, h] each).
 //
 // One CTA (256 threads) per 8 observation rows; activations in shared memory (89 kB), weights (1.2 MB, fp32) streamed from L2 with
 // every thread of a layer reading consecutive columns and using each weight for all 8 rows; 0.23 M MAC per row on the CUDA cores.
@@ -48,7 +51,16 @@ enum ValueRole {
   V_PROP_W = 0, V_PROP_B, V_ENC /* 28 */, V_CMD_W = V_ENC + 28, V_CMD_B, V_FC3_W, V_FC3_B, V_LSTM /* 9 */, V_OUT_W = V_LSTM + 9, V_OUT_B, V_N
 };
 static_assert(V_N == LLQ_HIER_ROLES_VALUE, "value-tower table (include/llq_policy.h)");
+// the strategic level's training table (arrays 2-50, then the heading logstd, array 96) takes the same place
+enum StrategicTrainRole {
+  SV_PROP_W = 0, SV_PROP_B, SV_ENC /* 24 + fusion fc 2 */, SV_PERC_W = SV_ENC + 26, SV_PERC_B, SV_GAME /* 3 fc: 6 */, SV_CAT_W = SV_GAME + 6,
+  SV_CAT_B, SV_LSTM /* 9 */, SV_OUT_W = SV_LSTM + 9, SV_OUT_B, SV_LOGSTD, SV_N
+};
+static_assert(SV_N == LLQ_HIER_ROLES_TRAIN_STRATEGIC, "strategic training table (include/llq_policy.h)");
 constexpr int RV = R_N_ALL;
+constexpr int kTrainRoles = (int)V_N > (int)SV_N ? (int)V_N : (int)SV_N;
+// kernel instances: deterministic (both levels), training at the environmental level, training at the strategic level
+enum Mode { M_DET = 0, M_TRAIN = 1, M_TRAIN_SEPMC = 2 };
 
 struct Net { const float* w; const int* off; };
 __device__ __forceinline__ const float* arr(const Net& n, int role) { return n.w + n.off[role]; }
@@ -56,7 +68,9 @@ __device__ __forceinline__ const float* arr(const Net& n, int role) { return n.w
 // out[r][j] = act(b[j] + sum_k in[r][k] W[k][j]) for the CTA's kRows rows; W row major [K][N], N a multiple of 4, every array 16-byte
 // aligned in the blob.  A thread owns FOUR consecutive columns of all rows (one 16-byte weight load and kRows shared-memory broadcasts
 // per 4 x kRows FMAs); the input dimension is split into `parts` interleaved slices over the thread groups, partial sums meet in `scratch`
-// (parts * kRows * N <= 4096 floats).
+// (parts * kRows * N <= 4096 floats).  ACC: the sums are added to what `out` holds (b unused), so a layer too wide for one input buffer
+// runs as two passes over K, the first without its activation.
+template <bool ACC = false>
 __device__ void dense(const float* in, int in_ld, int K, const float* W, const float* b, int N, float* out, int out_ld, float* scratch, bool relu) {
   const int t = threadIdx.x;
   const int quads = N >> 2;
@@ -98,7 +112,7 @@ __device__ void dense(const float* in, int in_ld, int K, const float* W, const f
   __syncthreads();
   for (int idx = t; idx < kRows * N; idx += kThreads) {
     const int r = idx / N, jj = idx - r * N;
-    float v = b ? b[jj] : 0.f;
+    float v = ACC ? out[r * out_ld + jj] : (b ? b[jj] : 0.f);
     for (int q = 0; q < parts; q++) v += scratch[(q * kRows + r) * N + jj];
     out[r * out_ld + jj] = relu ? fmaxf(v, 0.f) : v;
   }
@@ -268,14 +282,35 @@ __device__ __forceinline__ float gumbel(uint32_t r) {
   return -logf(-logf(u));
 }
 
-template <bool TRAIN>
+// Box-Muller pair of two Philox words with the conversions of llq_policy.cu's Gaussian action noise: u0 = (ra + 1/2) 2^-32 in fp32,
+// clamped below 1 (ra >= 2^32 - 128 rounds to 1.0f), u1 = rb 2^-32; returns sqrt(-2 log u0) (cos, sin)(2 pi u1).  (llq_policy.cu keeps
+// its inline form: calling this there changes that kernel's instruction schedule.)
+__device__ __forceinline__ float2 box_muller(uint32_t ra, uint32_t rb) {
+  const float u0 = ((float)ra + 0.5f) * 2.3283064365386963e-10f, u1 = (float)rb * 2.3283064365386963e-10f;
+  const float rad = sqrtf(-2.0f * logf(fminf(u0, 0.99999994f)));
+  float s, c;
+  sincosf(6.283185307179586f * u1, &s, &c);
+  return make_float2(rad * c, rad * s);
+}
+
+// the 29 game-vector slots of every row (percept_vec | oppo_info | flag_info | with_flag) -> x[r][0..29)
+__device__ __forceinline__ void game_vector(Smem& S) {
+  for (int idx = threadIdx.x; idx < kRows * 29; idx += kThreads) {
+    const int r = idx / 29, i = idx - r * 29;
+    S.x[r][i] = i < 5 ? S.obs[r][913 + i] : (i < 20 ? S.obs[r][918 + i - 5] : (i < 27 ? S.obs[r][948 + i - 20] : S.obs[r][962 + i - 27]));
+  }
+  __syncthreads();
+}
+
+template <int MODE>
 __global__ void __launch_bounds__(kThreads) hier_policy_kernel(Net net, int strategic, const float* __restrict__ obs, long long obs_ld, int n_rows,
                                                                const unsigned char* __restrict__ done, float* __restrict__ state, float* __restrict__ actions,
                                                                int* __restrict__ codes, float* __restrict__ heading, Sample smp) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   Smem& S = *reinterpret_cast<Smem*>(smem_raw);
   const int row0 = blockIdx.x * kRows, t = threadIdx.x;
-  if constexpr (TRAIN) strategic = 0;                       // the training instance serves the environmental level only
+  if constexpr (MODE == M_TRAIN) strategic = 0;
+  if constexpr (MODE == M_TRAIN_SEPMC) strategic = 1;
   const int ow = strategic ? 965 : 916;
   if (t < kRows) {
     const int live = row0 + t < n_rows;
@@ -292,18 +327,14 @@ __global__ void __launch_bounds__(kThreads) hier_policy_kernel(Net net, int stra
     S.p[r][i] = fminf(fmaxf((S.obs[r][i] - arr(net, R_MEAN)[i]) / (arr(net, R_STD)[i] + 1e-8f), -5.f), 5.f);
   }
   __syncthreads();
-  const int ssz = (TRAIN || strategic) ? 128 : 64;
+  const int ssz = MODE == M_TRAIN_SEPMC ? 192 : ((MODE == M_TRAIN || strategic) ? 128 : 64);
   float* st = state + (size_t)row0 * ssz;
   if (strategic) {
     // ---- heading controller
     dense(&S.p[0][0], 136, 135, arr(net, R_HPROP_W), arr(net, R_HPROP_B), 64, &S.cat[0][0], 256, S.scr, true);              // cat[0..64)
     perception(net, R_HENC, &S.obs[0][0], kObsLd, S.a, S.b, &S.x[0][0], 256);                                                // x[0..88)
     dense(&S.x[0][0], 256, 88, arr(net, R_HENC + 24), arr(net, R_HENC + 25), 64, &S.cat[0][64], 256, S.scr, true);          // cat[64..128)
-    for (int idx = t; idx < kRows * 29; idx += kThreads) {
-      const int r = idx / 29, i = idx - r * 29;
-      S.x[r][i] = i < 5 ? S.obs[r][913 + i] : (i < 20 ? S.obs[r][918 + i - 5] : (i < 27 ? S.obs[r][948 + i - 20] : S.obs[r][962 + i - 27]));
-    }
-    __syncthreads();
+    game_vector(S);
     dense(&S.x[0][0], 256, 29, arr(net, R_HVEC), arr(net, R_HVEC + 1), 64, &S.y[0][0], 256, S.scr, true);
     dense(&S.y[0][0], 256, 64, arr(net, R_HVEC + 2), arr(net, R_HVEC + 3), 64, &S.cat[0][128], 256, S.scr, true);           // cat[128..192)
     dense(&S.cat[0][0], 256, 192, arr(net, R_HEMB_W), arr(net, R_HEMB_B), 256, &S.x[0][0], 256, S.scr, true);
@@ -311,14 +342,28 @@ __global__ void __launch_bounds__(kThreads) hier_policy_kernel(Net net, int stra
     if (t < kRows) {
       float a = arr(net, R_HMU_B)[0];
       for (int k = 0; k < 32; k++) a = fmaf(S.h[t][k], arr(net, R_HMU_W)[k], a);
-      a = fminf(fmaxf(a, -3.14159265358979f), 3.14159265358979f);
-      S.ang[t] = a;
-      if (heading && S.live[t]) heading[row0 + t] = a;
+      if constexpr (MODE == M_TRAIN_SEPMC) {
+        // heading sample a = mu + exp(logstd) eps: eps from Philox keyed (global row, q = 64, counter) / seed (q 0..63 are the Gumbel draws'
+        // of the environmental level); the record gets the raw a and -log p of the raw a, the code controller the clipped one
+        const uint4 r = philox4x32(make_uint4((uint32_t)(smp.row_gid0 + row0 + t), 64u, (uint32_t)smp.counter, (uint32_t)(smp.counter >> 32)),
+                                   make_uint2((uint32_t)smp.seed, (uint32_t)(smp.seed >> 32)));
+        const float eps = box_muller(r.x, r.y).x, ls = arr(net, RV + SV_LOGSTD)[0];
+        a = fmaf(expf(ls), eps, a);
+        if (S.live[t]) {
+          if (heading) heading[(size_t)(row0 + t) * smp.out_ld] = a;
+          if (smp.neglogp) smp.neglogp[(size_t)(row0 + t) * smp.out_ld] = 0.5f * eps * eps + ls + 0.91893853320467274f;   // + 0.5 log(2 pi)
+        }
+        S.ang[t] = fminf(fmaxf(a, -3.14159265358979f), 3.14159265358979f);
+      } else {
+        a = fminf(fmaxf(a, -3.14159265358979f), 3.14159265358979f);
+        S.ang[t] = a;
+        if (heading && S.live[t]) heading[row0 + t] = a;
+      }
     }
     __syncthreads();
     st += 64;
   }
-  if constexpr (TRAIN) {
+  if constexpr (MODE == M_TRAIN) {
     // ---- value tower (arrays 2-46), wired like the code controller: [prop 135 -> 128 | command encoder -> 64 -> 128] -> 256 -> LSTM(32)
     // -> V (linear); its [c, h] is the second half of the row's state
     dense(&S.p[0][0], 136, 135, arr(net, RV + V_PROP_W), arr(net, RV + V_PROP_B), 128, &S.cat[0][0], 256, S.scr, true);       // cat[0..128)
@@ -340,6 +385,28 @@ __global__ void __launch_bounds__(kThreads) hier_policy_kernel(Net net, int stra
     }
     __syncthreads();
   }
+  if constexpr (MODE == M_TRAIN_SEPMC) {
+    // ---- value tower of the strategic level (arrays 2-50), in the heading controller's [prop | perception | game] order: prop 135 -> 128 |
+    // perception encoder 88 -> 64 -> 128 | game vector 29 -> 64 -> 64 -> 128, concatenated 384 -> 256 (two passes over K: cat holds 256)
+    // -> LSTM(32) -> V (linear); its [c, h] is the third part of the row's state
+    dense(&S.p[0][0], 136, 135, arr(net, RV + SV_PROP_W), arr(net, RV + SV_PROP_B), 128, &S.cat[0][0], 256, S.scr, true);     // cat[0..128)
+    perception(net, RV + SV_ENC, &S.obs[0][0], kObsLd, S.a, S.b, &S.x[0][0], 256);                                          // x[0..88)
+    dense(&S.x[0][0], 256, 88, arr(net, RV + SV_ENC + 24), arr(net, RV + SV_ENC + 25), 64, &S.y[0][0], 256, S.scr, true);    // y[0..64)
+    dense(&S.y[0][0], 256, 64, arr(net, RV + SV_PERC_W), arr(net, RV + SV_PERC_B), 128, &S.cat[0][128], 256, S.scr, true);   // cat[128..256)
+    game_vector(S);                                                                                                        // x[0..29)
+    dense(&S.x[0][0], 256, 29, arr(net, RV + SV_GAME), arr(net, RV + SV_GAME + 1), 64, &S.y[0][0], 256, S.scr, true);
+    dense(&S.y[0][0], 256, 64, arr(net, RV + SV_GAME + 2), arr(net, RV + SV_GAME + 3), 64, &S.x[0][0], 256, S.scr, true);
+    dense(&S.x[0][0], 256, 64, arr(net, RV + SV_GAME + 4), arr(net, RV + SV_GAME + 5), 128, &S.y[0][0], 256, S.scr, true);   // y[0..128)
+    dense(&S.cat[0][0], 256, 256, arr(net, RV + SV_CAT_W), arr(net, RV + SV_CAT_B), 256, &S.x[0][0], 256, S.scr, false);     // rows 0-255
+    dense<true>(&S.y[0][0], 256, 128, arr(net, RV + SV_CAT_W) + 256 * 256, nullptr, 256, &S.x[0][0], 256, S.scr, true);    // rows 256-383
+    lstm_step(net, RV + SV_LSTM, &S.x[0][0], st + 64, ssz, S.live, S.wipe, &S.zx[0][0], &S.zh[0][0], &S.c[0][0], &S.h[0][0], S.scr);
+    if (t < kRows) {
+      float v = arr(net, RV + SV_OUT_B)[0];
+      for (int k = 0; k < 32; k++) v = fmaf(S.h[t][k], arr(net, RV + SV_OUT_W)[k], v);
+      if (smp.values && S.live[t]) smp.values[(size_t)(row0 + t) * smp.out_ld] = v;
+    }
+    __syncthreads();
+  }
   // ---- code controller (environmental level)
   dense(&S.p[0][0], 136, 135, arr(net, R_MPROP_W), arr(net, R_MPROP_B), 64, &S.cat[0][0], 256, S.scr, true);                // cat[0..64)
   if (t < kRows * 3) {
@@ -353,7 +420,7 @@ __global__ void __launch_bounds__(kThreads) hier_policy_kernel(Net net, int stra
   dense(&S.cat[0][0], 256, 128, arr(net, R_MEMB_W), arr(net, R_MEMB_B), 256, &S.x[0][0], 256, S.scr, true);
   lstm_step(net, R_MLSTM, &S.x[0][0], st, ssz, S.live, S.wipe, &S.zx[0][0], &S.zh[0][0], &S.c[0][0], &S.h[0][0], S.scr);
   dense(&S.h[0][0], 32, 32, arr(net, R_LOGIT_W), arr(net, R_LOGIT_B), 256, &S.y[0][0], 256, S.scr, false);                  // logits
-  if constexpr (TRAIN) {
+  if constexpr (MODE == M_TRAIN) {
     // Gumbel-max sample: code = argmax_j (logit_j + g_j), g from Philox keyed (global row, q, counter) / seed, one call per four logits
     for (int idx = t; idx < kRows * 64; idx += kThreads) {
       const int r = idx >> 6, q = idx & 63;
@@ -422,15 +489,16 @@ struct llq_hier_policy {
 
 namespace {
 
-// `value_offsets` (LLQ_HIER_ROLES_VALUE entries) null: a deterministic handle
-int create(const float* weights, int64_t n_weights, const int32_t* offsets, int32_t n_roles, const int32_t* value_offsets, int32_t strategic,
-           int32_t device, llq_hier_policy_handle* out) {
+// `value_offsets` (n_value entries: LLQ_HIER_ROLES_VALUE, or LLQ_HIER_ROLES_TRAIN_STRATEGIC at the strategic level) null: a deterministic
+// handle
+int create(const float* weights, int64_t n_weights, const int32_t* offsets, int32_t n_roles, const int32_t* value_offsets, int32_t n_value,
+           int32_t strategic, int32_t device, llq_hier_policy_handle* out) {
   if (!weights || !offsets || !out) return fail_h(LLQ_EINVAL, "null argument");
   if (n_roles != (strategic ? LLQ_HIER_ROLES_ALL : LLQ_HIER_ROLES_MLC)) return fail_h(LLQ_EINVAL, "role table has the wrong length (include/llq_policy.h)");
   for (int i = 0; i < n_roles; i++) if (offsets[i] < 0 || offsets[i] >= n_weights) return fail_h(LLQ_EINVAL, "role offset outside the weight blob");
   if (value_offsets)
-    for (int i = 0; i < LLQ_HIER_ROLES_VALUE; i++)
-      if (value_offsets[i] < 0 || value_offsets[i] >= n_weights) return fail_h(LLQ_EINVAL, "value-tower offset outside the weight blob");
+    for (int i = 0; i < n_value; i++)
+      if (value_offsets[i] < 0 || value_offsets[i] >= n_weights) return fail_h(LLQ_EINVAL, "training-table offset outside the weight blob");
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail_h(LLQ_ECUDA, "no CUDA device visible (no CPU fallback)");
   if (device < 0 || device >= ndev) return fail_h(LLQ_EINVAL, "device ordinal out of range");
@@ -438,9 +506,9 @@ int create(const float* weights, int64_t n_weights, const int32_t* offsets, int3
   llq_hier_policy* h = new (std::nothrow) llq_hier_policy();
   if (!h) return fail_h(LLQ_ENOMEM, "out of memory");
   h->device = device; h->strategic = strategic ? 1 : 0; h->train = value_offsets ? 1 : 0;
-  std::vector<int> off(RV + V_N, 0);
+  std::vector<int> off(RV + kTrainRoles, 0);
   for (int i = 0; i < n_roles; i++) off[i] = offsets[i];
-  if (value_offsets) for (int i = 0; i < V_N; i++) off[RV + i] = value_offsets[i];
+  if (value_offsets) for (int i = 0; i < n_value; i++) off[RV + i] = value_offsets[i];
   if (cudaMalloc(&h->d_w, sizeof(float) * (size_t)n_weights) != cudaSuccess || cudaMalloc(&h->d_off, sizeof(int) * off.size()) != cudaSuccess ||
       cudaMemcpy(h->d_w, weights, sizeof(float) * (size_t)n_weights, cudaMemcpyHostToDevice) != cudaSuccess ||
       cudaMemcpy(h->d_off, off.data(), sizeof(int) * off.size(), cudaMemcpyHostToDevice) != cudaSuccess) {
@@ -451,18 +519,19 @@ int create(const float* weights, int64_t n_weights, const int32_t* offsets, int3
   return LLQ_OK;
 }
 
-template <bool TRAIN>
+template <int MODE>
 int launch(llq_hier_policy_handle h, const float* d_obs, int64_t obs_ld, int32_t n, const uint8_t* d_done, float* d_state, float* d_actions,
            int32_t* d_codes, float* d_heading, const Sample& smp, void* stream) {
   if (cudaSetDevice(h->device) != cudaSuccess) return fail_h(LLQ_ECUDA, "cudaSetDevice failed");
   Net net{h->d_w, h->d_off};
   if (!h->attr_set) {
-    if (cudaFuncSetAttribute(hier_policy_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem)) != cudaSuccess ||
-        (h->train && cudaFuncSetAttribute(hier_policy_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem)) != cudaSuccess))
+    if (cudaFuncSetAttribute(hier_policy_kernel<M_DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem)) != cudaSuccess ||
+        (h->train && cudaFuncSetAttribute(h->strategic ? hier_policy_kernel<M_TRAIN_SEPMC> : hier_policy_kernel<M_TRAIN>,
+                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem)) != cudaSuccess))
       return fail_h(LLQ_ECUDA, "cudaFuncSetAttribute failed");
     h->attr_set = true;                                      // per handle = per device
   }
-  hier_policy_kernel<TRAIN><<<(n + kRows - 1) / kRows, kThreads, sizeof(Smem), (cudaStream_t)stream>>>(net, h->strategic, d_obs, obs_ld, n, d_done, d_state,
+  hier_policy_kernel<MODE><<<(n + kRows - 1) / kRows, kThreads, sizeof(Smem), (cudaStream_t)stream>>>(net, h->strategic, d_obs, obs_ld, n, d_done, d_state,
                                                                                                     d_actions, d_codes, d_heading, smp);
   if (cudaGetLastError() != cudaSuccess) return fail_h(LLQ_ECUDA, "hier_policy_kernel launch failed");
   return LLQ_OK;
@@ -474,15 +543,24 @@ extern "C" {
 
 int llq_hier_policy_create(const float* weights, int64_t n_weights, const int32_t* offsets, int32_t n_roles, int32_t strategic, int32_t device,
                            llq_hier_policy_handle* out) {
-  return create(weights, n_weights, offsets, n_roles, nullptr, strategic, device, out);
+  return create(weights, n_weights, offsets, n_roles, nullptr, 0, strategic, device, out);
 }
 
 int llq_hier_policy_create_train(const float* weights, int64_t n_weights, const int32_t* offsets, int32_t n_roles, const int32_t* value_offsets,
                                  int32_t n_value_roles, int32_t strategic, int32_t device, llq_hier_policy_handle* out) {
-  if (strategic) return fail_h(LLQ_EUNSUPPORTED, "training rollouts exist for the environmental level only (include/llq_policy.h)");
+  if (strategic)
+    return fail_h(LLQ_EUNSUPPORTED, "this entry creates training handles for the environmental level only; the strategic level's is "
+                                    "llq_hier_policy_create_train_strategic (include/llq_policy.h)");
   if (!value_offsets) return fail_h(LLQ_EINVAL, "null argument");
   if (n_value_roles != LLQ_HIER_ROLES_VALUE) return fail_h(LLQ_EINVAL, "value-tower table has the wrong length (include/llq_policy.h)");
-  return create(weights, n_weights, offsets, n_roles, value_offsets, 0, device, out);
+  return create(weights, n_weights, offsets, n_roles, value_offsets, LLQ_HIER_ROLES_VALUE, 0, device, out);
+}
+
+int llq_hier_policy_create_train_strategic(const float* weights, int64_t n_weights, const int32_t* offsets, int32_t n_roles,
+                                           const int32_t* train_offsets, int32_t n_train_roles, int32_t device, llq_hier_policy_handle* out) {
+  if (!train_offsets) return fail_h(LLQ_EINVAL, "null argument");
+  if (n_train_roles != LLQ_HIER_ROLES_TRAIN_STRATEGIC) return fail_h(LLQ_EINVAL, "strategic training table has the wrong length (include/llq_policy.h)");
+  return create(weights, n_weights, offsets, n_roles, train_offsets, LLQ_HIER_ROLES_TRAIN_STRATEGIC, 1, device, out);
 }
 
 int llq_hier_policy_destroy(llq_hier_policy_handle h) {
@@ -496,9 +574,11 @@ int llq_hier_policy_destroy(llq_hier_policy_handle h) {
 int llq_hier_policy_forward(llq_hier_policy_handle h, const float* d_obs, int64_t obs_ld, int32_t n, const uint8_t* d_done, float* d_state,
                             float* d_actions, int32_t* d_codes, float* d_heading, void* stream) {
   if (!h || !d_obs || !d_state || !d_actions) return fail_h(LLQ_EINVAL, "null argument");
-  if (h->train) return fail_h(LLQ_EINVAL, "a training handle steps with llq_hier_policy_forward_rec (its state rows are 128 floats)");
+  if (h->train)
+    return fail_h(LLQ_EINVAL, h->strategic ? "a strategic training handle steps with llq_hier_policy_forward_rec_strategic (its state rows are 192 floats)"
+                                           : "a training handle steps with llq_hier_policy_forward_rec (its state rows are 128 floats)");
   if (n <= 0 || obs_ld < (h->strategic ? 965 : 916)) return fail_h(LLQ_EINVAL, "bad row count or row stride");
-  return launch<false>(h, d_obs, obs_ld, n, d_done, d_state, d_actions, d_codes, d_heading, Sample{}, stream);
+  return launch<M_DET>(h, d_obs, obs_ld, n, d_done, d_state, d_actions, d_codes, d_heading, Sample{}, stream);
 }
 
 int llq_hier_policy_forward_rec(llq_hier_policy_handle h, const float* d_obs, int64_t obs_ld, int32_t n, const uint8_t* d_done, float* d_state,
@@ -506,9 +586,20 @@ int llq_hier_policy_forward_rec(llq_hier_policy_handle h, const float* d_obs, in
                                 int64_t row_gid0, void* stream) {
   if (!h || !d_obs || !d_state || !d_actions) return fail_h(LLQ_EINVAL, "null argument");
   if (!h->train) return fail_h(LLQ_EINVAL, "not a training handle (llq_hier_policy_create_train)");
+  if (h->strategic) return fail_h(LLQ_EINVAL, "a strategic training handle steps with llq_hier_policy_forward_rec_strategic");
   if (n <= 0 || obs_ld < 916 || out_ld < 1) return fail_h(LLQ_EINVAL, "bad row count or row stride");
   const Sample smp{d_values, d_neglogp, (long long)out_ld, (unsigned long long)seed, (unsigned long long)counter, (long long)row_gid0};
-  return launch<true>(h, d_obs, obs_ld, n, d_done, d_state, d_actions, d_codes, nullptr, smp, stream);
+  return launch<M_TRAIN>(h, d_obs, obs_ld, n, d_done, d_state, d_actions, d_codes, nullptr, smp, stream);
+}
+
+int llq_hier_policy_forward_rec_strategic(llq_hier_policy_handle h, const float* d_obs, int64_t obs_ld, int32_t n, const uint8_t* d_done,
+                                          float* d_state, float* d_actions, int32_t* d_codes, float* d_heading, float* d_values, float* d_neglogp,
+                                          int64_t out_ld, uint64_t seed, uint64_t counter, int64_t row_gid0, void* stream) {
+  if (!h || !d_obs || !d_state || !d_actions) return fail_h(LLQ_EINVAL, "null argument");
+  if (!h->train || !h->strategic) return fail_h(LLQ_EINVAL, "not a strategic training handle (llq_hier_policy_create_train_strategic)");
+  if (n <= 0 || obs_ld < 965 || out_ld < 1) return fail_h(LLQ_EINVAL, "bad row count or row stride");
+  const Sample smp{d_values, d_neglogp, (long long)out_ld, (unsigned long long)seed, (unsigned long long)counter, (long long)row_gid0};
+  return launch<M_TRAIN_SEPMC>(h, d_obs, obs_ld, n, d_done, d_state, d_actions, d_codes, d_heading, smp, stream);
 }
 
 const char* llq_hier_policy_last_error(void) { return g_err_h.c_str(); }

@@ -26,7 +26,8 @@ import numpy as np
 import torch
 
 from .trajectory import (ACT_DIM, COL_ACTION, COL_DONE, COL_NEGLOGP, COL_REWARD, COL_VALUE, HCOL_CODE, HCOL_DONE, HCOL_NEGLOGP, HCOL_REWARD,
-                         HCOL_VALUE, HIER_TRAJ_WIDTH, OBS_DIM, TRAJ_WIDTH)
+                         HCOL_VALUE, HIER_TRAJ_WIDTH, OBS_DIM, SCOL_CODE, SCOL_DONE, SCOL_HEADING, SCOL_NEGLOGP, SCOL_REWARD, SCOL_VALUE,
+                         SEPMC_TRAJ_WIDTH, TRAJ_WIDTH)
 
 OBS_LEAVES = OrderedDict([("prop", 99), ("prop_a", 36), ("future", 72)])        # PLE:117-124
 # leaf order of a flattened PMCInputs record (namedtuple order, the observation dict in key-insertion order)
@@ -85,27 +86,60 @@ def hier_slab_records(slab, initial_state, first_mask, bootstrap_value, gamma=GA
     M[t] = done[t-1]) -- all [T, N] float32 -- and `S` [N, 128], the recurrent state the unroll started from (code LSTM [c, h], then
     value LSTM [c, h])."""
     assert slab.dim() == 3 and slab.shape[2] == HIER_TRAJ_WIDTH, "expected a [T, N, %d] trajectory slab" % HIER_TRAJ_WIDTH
-    T, N, _ = slab.shape
+    out = _recurrent_records(slab, HIER_OBS_LEAVES, slab[:, :, HCOL_DONE], slab[:, :, HCOL_REWARD], slab[:, :, HCOL_VALUE], first_mask,
+                             bootstrap_value, gamma, lam)
+    head = OrderedDict((k, out.pop(k)) for k in HIER_OBS_LEAVES)
+    head["A_Z"] = slab[:, :, HCOL_CODE].to(torch.int64)
+    head["neglogp"] = slab[:, :, HCOL_NEGLOGP]
+    head.update(out)
+    head["S"] = initial_state
+    return head
+
+
+# observation leaves of the strategic level (CTG:111-124), in the order of its 965 observation columns
+SEPMC_OBS_LEAVES = OrderedDict([("prop", (99,)), ("prop_a", (36,)), ("percept_2d", (25, 13)), ("percept_1d", (128,)), ("percept_front", (25, 13)),
+                                ("percept_vec", (5,)), ("oppo_info", (15,)), ("oppo_info_cheat", (15,)), ("flag_info", (7,)),
+                                ("flag_info_cheat", (7,)), ("with_flag", (2,)), ("control_spd", (1,))])
+
+
+def _recurrent_records(slab, leaves, done, r, v, first_mask, bootstrap_value, gamma, lam):
+    """The observation leaves [T, N, *leaf] and discount, r, V, R (lambda-returns), M (the mask each forward received) of an unroll."""
+    T, N = done.shape
     out = OrderedDict()
     c = 0
-    for name, shape in HIER_OBS_LEAVES.items():
+    for name, shape in leaves.items():
         k = int(np.prod(shape))
         out[name] = slab[:, :, c:c + k].reshape(T, N, *shape)
         c += k
-    r, done, v = slab[:, :, HCOL_REWARD], slab[:, :, HCOL_DONE], slab[:, :, HCOL_VALUE]
     discount = gamma * (1.0 - done)
-    out["A_Z"] = slab[:, :, HCOL_CODE].to(torch.int64)
-    out["neglogp"] = slab[:, :, HCOL_NEGLOGP]
-    out["discount"] = discount
-    out["r"] = r
-    out["V"] = v
+    out["discount"], out["r"], out["V"] = discount, r, v
     out["R"] = lambda_returns(r, discount, v, bootstrap_value.to(slab.dtype), lam)
     mask = torch.empty((T, N), dtype=slab.dtype, device=slab.device)
     mask[0] = (first_mask != 0).to(slab.dtype)
     mask[1:] = (done[:-1] != 0).to(slab.dtype)
     out["M"] = mask
-    out["S"] = initial_state
     return out
+
+
+def sepmc_slab_records(slab, initial_state, first_mask, bootstrap_value, gamma=GAMMA, lam=LAM):
+    """Learner tensors of a strategic-level unroll (`SepmcRolloutWorker.finish_unroll()`) for the learning robot (seat 0: rows 0, 2, 4, ...
+    of the `[T, 2P, 984]` slab), on the slab's device, named: the twelve observation leaves [T, P, *leaf] (CTG:111-124), `A_HLC` [T, P]
+    (the raw sampled heading), `A_Z` [T, P] int64 (the argmax code), `neglogp` (of the heading), `discount` = gamma (1 - done), `r`, `V`,
+    `R` (lambda-returns, bootstrapped with V(observation T)), `M` [T, P] = the mask each forward received (M[0] = first_mask, M[t] =
+    done[t-1]) -- all [T, P] float32 but A_Z -- and `S` [P, 192], the recurrent state the unroll started from (heading, code and value
+    LSTM, [c, h] each)."""
+    assert slab.dim() == 3 and slab.shape[2] == SEPMC_TRAJ_WIDTH and slab.shape[1] % 2 == 0, \
+        "expected a [T, 2P, %d] trajectory slab" % SEPMC_TRAJ_WIDTH
+    s0 = slab[:, 0::2]
+    out = _recurrent_records(s0, SEPMC_OBS_LEAVES, s0[:, :, SCOL_DONE], s0[:, :, SCOL_REWARD], s0[:, :, SCOL_VALUE], first_mask, bootstrap_value,
+                             gamma, lam)
+    head = OrderedDict((k, out.pop(k)) for k in SEPMC_OBS_LEAVES)
+    head["A_HLC"] = s0[:, :, SCOL_HEADING]
+    head["A_Z"] = s0[:, :, SCOL_CODE].to(torch.int64)
+    head["neglogp"] = s0[:, :, SCOL_NEGLOGP]
+    head.update(out)
+    head["S"] = initial_state
+    return head
 
 
 def slab_to_unrolls(slab, model_key, infos=None, **kw):

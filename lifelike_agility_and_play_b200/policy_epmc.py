@@ -223,15 +223,19 @@ class SepmcPolicy:
     prop 135 -> 64 | perception 88 -> 64 | game vector 29 -> 64 -> 64, concat 192 -> 256 -> LSTM(32) -> heading angle, clipped to +-pi),
     whose (cos, sin) joins the commanded speed as the `target_info` of the environmental-level encoder (`mlc_encoder`, :176-203) -> 256-way
     code -> the frozen primitive-level decoder.  `weights` = the 152 arrays of ``strategic_level.model``:
-    0-1 rms | 2-50 value tower | 51-96 heading controller | 97-139 code controller | 140 codebook | 141-150 decoder | 151 logstd."""
+    0-1 rms | 2-50 value tower | 51-96 heading controller (96: the heading's logstd) | 97-139 code controller | 140 codebook |
+    141-150 decoder | 151 logstd."""
 
     def __init__(self, weights):
         w = [np.asarray(a, np.float32) for a in weights]
         assert len(w) == 152 and w[83].shape == (192, 256) and w[140].shape == (32, 256), "not a strategic-level model"
         self.mean, self.std = w[0], w[1]
+        self.vf_prop, self.vf_percept, self.vf_perc_fc = (w[2], w[3]), CommandEncoder(w[4:30]), (w[30], w[31])
+        self.vf_game = [(w[32], w[33]), (w[34], w[35]), (w[36], w[37])]
+        self.vf_cat, self.vf_lstm, self.vf_out = (w[38], w[39]), LnLstm(w[40:49]), (w[49], w[50])
         self.h_prop, self.h_percept = (w[51], w[52]), CommandEncoder(w[53:79])
         self.h_vec = [(w[79], w[80]), (w[81], w[82])]
-        self.h_embed, self.h_lstm, self.h_mu = (w[83], w[84]), LnLstm(w[85:94]), (w[94], w[95])
+        self.h_embed, self.h_lstm, self.h_mu, self.h_logstd = (w[83], w[84]), LnLstm(w[85:94]), (w[94], w[95]), w[96]
         self.m_prop, self.m_cmd, self.m_embed = (w[97], w[98]), CommandEncoder(w[99:127]), (w[127], w[128])
         self.m_lstm, self.logits = LnLstm(w[129:138]), (w[138], w[139])
         self.codebook = w[140]
@@ -242,18 +246,57 @@ class SepmcPolicy:
     def initial_state(self, n):
         return np.zeros((n, 4 * self.nh), np.float32)          # [c, h] of the heading LSTM, then of the code LSTM
 
-    def act(self, obs, state, mask, return_aux=False):
+    def _split(self, obs):
         o = np.asarray(obs, np.float32)
         prop, p2d, p1d, pfr = o[:, 0:135], o[:, 135:460].reshape(-1, 25, 13), o[:, 460:588], o[:, 588:913].reshape(-1, 25, 13)
         game = np.concatenate([o[:, 913:918], o[:, 918:933], o[:, 948:955], o[:, 962:964]], axis=1)      # percept_vec | oppo_info | flag_info | with_flag
-        spd = o[:, 964:965]
-        mask = np.asarray(mask, np.float32)
         p = np.clip((prop - self.mean) / (self.std + 1e-8), -5.0, 5.0)
+        return p, p2d, p1d, pfr, game, o[:, 964:965]
+
+    def value(self, obs, state, mask):
+        """V(obs) of the value tower (arrays 2-50), state [N, 64] = [c, h] of its own LSTM, mask as in `act`.  Returns (V [N], new state).
+
+        The wiring is read off the array shapes with the heading controller's [prop | perception | game] order (the actor's value head of
+        example_sepmc_train.sh; sepmc_net.py's value part is not in the reference tree):
+            v1 = relu(p W2 + b3)                            135 -> 128
+            v2 = relu(usr_cmd_encoder(arrays 4-29) W30 + b31)    perception 88 -> 64 (no target), then 64 -> 128
+            v3 = game vector 29 -> 64 -> 64 -> 128          arrays 32-37, ReLU
+            v4 = relu([v1 | v2 | v3] W38 + b39)             384 -> 256
+            (c, h) = layer-norm LSTM(arrays 40-48)          state [c, h], zeroed where mask is set
+            V  = h W49 + b50                                32 -> 1, linear
+        Nothing pins this against TensorFlow here; it is the statement the device's strategic training forward
+        (llq_hier_policy_forward_rec_strategic) is checked against."""
+        p, p2d, p1d, pfr, game, _ = self._split(obs)
+        relu = lambda x: np.maximum(x, 0.0)
+        v1 = relu(p @ self.vf_prop[0] + self.vf_prop[1])
+        v2 = relu(self.vf_percept(p2d, p1d, pfr) @ self.vf_perc_fc[0] + self.vf_perc_fc[1])
+        v3 = game
+        for W, b in self.vf_game:
+            v3 = relu(v3 @ W + b)
+        v4 = relu(np.concatenate([v1, v2, v3], axis=1) @ self.vf_cat[0] + self.vf_cat[1])
+        h, state = self.vf_lstm.step(v4, state, np.asarray(mask, np.float32))
+        return (h @ self.vf_out[0] + self.vf_out[1])[:, 0].astype(np.float32), state
+
+    def act(self, obs, state, mask, return_aux=False, eps=None, return_neglogp=False):
+        """obs [N, 965], state [N, 128] ([c, h] of the heading LSTM, then of the code LSTM), mask [N] = 1 where the observation is the
+        first of an episode.  Returns (action [N, 12], new state), then (heading, code) with `return_aux`.  Without `eps` the heading is
+        the mean, clipped to +-pi.  `eps` [N]: the heading is SAMPLED, a = mean + exp(logstd) eps (the training actor's behaviour; the
+        device's training forward draws eps by Box-Muller from Philox, include/llq_policy.h); the code controller receives clip(a, +-pi),
+        and the returned heading is the raw a; `return_neglogp` appends -log p(a) = 0.5 eps^2 + logstd + 0.5 log(2 pi)."""
+        p, p2d, p1d, pfr, game, spd = self._split(obs)
+        mask = np.asarray(mask, np.float32)
         relu = lambda x: np.maximum(x, 0.0)
         ge = relu(relu(game @ self.h_vec[0][0] + self.h_vec[0][1]) @ self.h_vec[1][0] + self.h_vec[1][1])
         e = relu(np.concatenate([relu(p @ self.h_prop[0] + self.h_prop[1]), self.h_percept(p2d, p1d, pfr), ge], axis=1) @ self.h_embed[0] + self.h_embed[1])
         hh, s_h = self.h_lstm.step(e, state[:, :2 * self.nh], mask)
-        ang = np.clip(hh @ self.h_mu[0] + self.h_mu[1], -np.pi, np.pi)
+        mu = hh @ self.h_mu[0] + self.h_mu[1]
+        if eps is None:
+            ang = head = np.clip(mu, -np.pi, np.pi)
+        else:
+            eps = np.asarray(eps, np.float64).reshape(-1, 1)
+            ls = float(self.h_logstd.reshape(-1)[0])
+            head = (mu + np.exp(ls) * eps).astype(np.float32)
+            ang = np.clip(head, -np.float32(np.pi), np.float32(np.pi))
         tgt = np.concatenate([np.cos(ang), np.sin(ang), spd], axis=1).astype(np.float32)
         e2 = relu(np.concatenate([relu(p @ self.m_prop[0] + self.m_prop[1]), self.m_cmd(p2d, p1d, pfr, tgt)], axis=1) @ self.m_embed[0] + self.m_embed[1])
         hm, s_m = self.m_lstm.step(e2, state[:, 2 * self.nh:], mask)
@@ -264,7 +307,11 @@ class SepmcPolicy:
         x = relu(x @ self.dec[1][0] + self.dec[1][1])
         act = (x @ self.dec[2][0] + self.dec[2][1]).astype(np.float32)
         new_state = np.concatenate([s_h, s_m], axis=1)
-        return (act, new_state, ang[:, 0], code) if return_aux else (act, new_state)
+        out = (act, new_state) + ((head[:, 0], code) if return_aux else ())
+        if return_neglogp:
+            assert eps is not None, "-log p is that of a sampled heading: pass eps"
+            out += (0.5 * eps[:, 0] ** 2 + ls + 0.5 * np.log(2.0 * np.pi),)
+        return out
 
 
 _ENC = [(1, 1, 1, 4), (4,), (4, 4, 4, 4), (4,), (2, 2, 4, 4), (4,), (2, 2, 4, 1), (1,), (4, 1, 4), (4,), (4, 4, 4), (4,), (4, 4, 4), (4,), (4, 4, 1), (1,),
@@ -293,10 +340,11 @@ def random_weights(strategic=False, seed=0):
 # ---------------------------------------------------------------------------------------------------------------- device side
 def hier_role_arrays(strategic, value_tower=False):
     """Index (in the shipped file's array list) of the array that plays each role of include/llq_policy.h; `value_tower`: the
-    environmental level's value-tower table (LLQ_HIER_ROLES_VALUE entries) instead."""
+    environmental level's value-tower table (LLQ_HIER_ROLES_VALUE entries) instead (the strategic level's training table is
+    `strategic_train_role_arrays`)."""
     if value_tower:
         if strategic:
-            raise ValueError("the value-tower table exists for the environmental level only")
+            raise ValueError("the value-tower table exists for the environmental level only (strategic level: strategic_train_role_arrays)")
         return list(range(2, 47))
     if not strategic:
         return [0, 1, 47, 48] + list(range(49, 77)) + [77, 78] + list(range(79, 88)) + [88, 89, 90] + list(range(91, 101))
@@ -305,27 +353,44 @@ def hier_role_arrays(strategic, value_tower=False):
     return mlc + hlc
 
 
+def strategic_train_role_arrays():
+    """The strategic level's training table (LLQ_HIER_ROLES_TRAIN_STRATEGIC entries, include/llq_policy.h): the value tower, arrays
+    2-50 of strategic_level.model, then the heading logstd (array 96)."""
+    return list(range(2, 51)) + [96]
+
+
+def _policy_lib():
+    import ctypes as C
+    import os
+    from .policy import POLICY_LIB_PATH
+    if not os.path.exists(POLICY_LIB_PATH):
+        raise RuntimeError("%s is not built (python -c 'import __graft_entry__ as g; g.build()'); there is no CPU fallback" % POLICY_LIB_PATH)
+    lib = C.CDLL(POLICY_LIB_PATH)
+    lib.llq_hier_policy_last_error.restype = C.c_char_p
+    return lib
+
+
+def _weight_blob(weights):
+    """(blob, starts): the arrays concatenated as fp32, each starting on a 16-byte boundary (the kernel's float4 loads)."""
+    w = [np.ascontiguousarray(a, np.float32).reshape(-1) for a in weights]
+    w = [np.concatenate([a, np.zeros((-a.size) % 4, np.float32)]) for a in w]
+    starts = np.concatenate([[0], np.cumsum([a.size for a in w])]).astype(np.int64)
+    return np.concatenate(w), starts
+
+
 class DeviceHierPolicy:
     """The environmental- / strategic-level policy on the GPU (csrc/llq_policy_hier.cu through include/llq_policy.h): reads the engine's
     observation rows in place, keeps the LSTM states on the device, writes the actions the fused env step consumes.
     `train=True` (environmental level only): the training handle, stepped with `forward_rec` (sampled code, -log p, V; state rows of
-    128 floats = code LSTM, then value LSTM)."""
+    128 floats = code LSTM, then value LSTM); the strategic level's training handle is `DeviceSepmcTrainPolicy`."""
 
     def __init__(self, weights, device=0, train=False):
         import ctypes as C
-        from .policy import POLICY_LIB_PATH
-        import os
-        if not os.path.exists(POLICY_LIB_PATH):
-            raise RuntimeError("%s is not built (python -c 'import __graft_entry__ as g; g.build()'); there is no CPU fallback" % POLICY_LIB_PATH)
-        self._C, self.lib = C, C.CDLL(POLICY_LIB_PATH)
-        w = [np.ascontiguousarray(a, np.float32).reshape(-1) for a in weights]
-        self.strategic = len(w) == 152
-        assert len(w) in (102, 152), "expected an environmental-level (102 arrays) or a strategic-level (152 arrays) model"
-        w = [np.concatenate([a, np.zeros((-a.size) % 4, np.float32)]) for a in w]        # every array starts on a 16-byte boundary (float4 loads)
-        starts = np.concatenate([[0], np.cumsum([a.size for a in w])]).astype(np.int64)
-        blob = np.concatenate(w)
+        self._C, self.lib = C, _policy_lib()
+        self.strategic = len(weights) == 152
+        assert len(weights) in (102, 152), "expected an environmental-level (102 arrays) or a strategic-level (152 arrays) model"
+        blob, starts = _weight_blob(weights)
         off = np.array([starts[i] for i in hier_role_arrays(self.strategic)], np.int32)
-        self.lib.llq_hier_policy_last_error.restype = C.c_char_p
         h = C.c_void_p()
         self.train = bool(train)
         if self.train:
@@ -365,3 +430,40 @@ class DeviceHierPolicy:
         if self._h:
             self.lib.llq_hier_policy_destroy(self._h)
             self._h = None
+
+
+class DeviceSepmcTrainPolicy(DeviceHierPolicy):
+    """The strategic level's training handle on the GPU (include/llq_policy.h, llq_hier_policy_create_train_strategic): `forward_rec`
+    samples the heading, writes it raw with its -log p and V, and runs the frozen code controller (argmax code) and decoder on the
+    clipped heading.  State rows of 192 floats: heading LSTM, code LSTM, value LSTM ([c, h] each)."""
+
+    def __init__(self, weights, device=0):
+        import ctypes as C
+        self._C, self.lib = C, _policy_lib()
+        assert len(weights) == 152, "expected a strategic-level model (152 arrays)"
+        self.strategic, self.train = True, True
+        blob, starts = _weight_blob(weights)
+        off = np.array([starts[i] for i in hier_role_arrays(True)], np.int32)
+        toff = np.array([starts[i] for i in strategic_train_role_arrays()], np.int32)
+        h = C.c_void_p()
+        rc = self.lib.llq_hier_policy_create_train_strategic(blob.ctypes.data_as(C.c_void_p), C.c_int64(blob.size), off.ctypes.data_as(C.c_void_p),
+                                                             C.c_int32(off.size), toff.ctypes.data_as(C.c_void_p), C.c_int32(toff.size),
+                                                             C.c_int32(device), C.byref(h))
+        if rc:
+            raise RuntimeError("llq_hier_policy_create_train_strategic: %s" % self.lib.llq_hier_policy_last_error().decode())
+        self._h = h
+        self.state_dim, self.obs_dim = 192, 965
+
+    def forward_rec(self, obs_ptr, obs_ld, n, done_ptr, state_ptr, act_ptr, codes_ptr, heading_ptr, values_ptr, neglogp_ptr, out_ld, seed, counter,
+                    row_gid0=0, stream=None):
+        """Training step (include/llq_policy.h, llq_hier_policy_forward_rec_strategic): raw sampled heading / V / -log p of row i ->
+        heading_ptr / values_ptr / neglogp_ptr + i * out_ld floats, argmax code -> codes_ptr (int32); the heading noise is keyed by
+        (row_gid0 + i, counter) and `seed`."""
+        C = self._C
+        rc = self.lib.llq_hier_policy_forward_rec_strategic(self._h, C.c_void_p(obs_ptr), C.c_int64(obs_ld), C.c_int32(n), C.c_void_p(done_ptr or 0),
+                                                            C.c_void_p(state_ptr), C.c_void_p(act_ptr), C.c_void_p(codes_ptr or 0),
+                                                            C.c_void_p(heading_ptr or 0), C.c_void_p(values_ptr or 0), C.c_void_p(neglogp_ptr or 0),
+                                                            C.c_int64(out_ld), C.c_uint64(seed), C.c_uint64(counter), C.c_int64(row_gid0),
+                                                            C.c_void_p(stream or 0))
+        if rc:
+            raise RuntimeError("llq_hier_policy_forward_rec_strategic: %s" % self.lib.llq_hier_policy_last_error().decode())
