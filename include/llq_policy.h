@@ -123,6 +123,30 @@ int llq_hier_policy_forward_rec(llq_hier_policy_handle h, const float* d_obs, in
 int llq_hier_policy_forward_rec_strategic(llq_hier_policy_handle h, const float* d_obs, int64_t obs_ld, int32_t n, const uint8_t* d_done,
                                           float* d_state, float* d_actions, int32_t* d_codes, float* d_heading, float* d_values, float* d_neglogp,
                                           int64_t out_ld, uint64_t seed, uint64_t counter, int64_t row_gid0, void* stream);
+/* ---- opponent pool: K deterministic strategic-level models in one handle, every row run with its own model in one launch (a league
+ * actor draws its frozen opponent per game; this is that draw for a whole batch of pairs).  A pool handle is refused by the other
+ * forward entries and is single-owner: it holds one workspace, so two streams must not run llq_hier_policy_forward_pool on it at once.
+ * Create: `weights` holds all K models; `offsets` [n_models * LLQ_HIER_ROLES_ALL], model k's 101-role table of llq_hier_policy_create
+ * (strategic level) at offsets + k * LLQ_HIER_ROLES_ALL, absolute into `weights`; 1 <= n_models <= LLQ_HIER_POOL_MAX; `max_rows` bounds
+ * n of every forward.  Null arguments, a bad count or an offset outside the blob return LLQ_EINVAL before the device is touched.  The
+ * draw probabilities start uniform. */
+#define LLQ_HIER_POOL_MAX 64
+int llq_hier_policy_create_pool(const float* weights, int64_t n_weights, const int32_t* offsets, int32_t n_models, int32_t max_rows, int32_t device,
+                                llq_hier_policy_handle* out);
+/* Draw probabilities of the next forwards (n must equal n_models; every entry finite and >= 0, their sum > 0; else LLQ_EINVAL): the
+ * host forms, in fp64, cum_k = p_0 + ... + p_k summed in order and the cutoffs t_k = floor(cum_k / cum_{K-1} * 2^32), t_{K-1} = 2^32; a
+ * model with p = 0 is never drawn.  The cutoffs go to the next launch by value: no device copy, so a call between two steps is safe. */
+int llq_hier_policy_set_pool_probs(llq_hier_policy_handle h, const double* probs, int32_t n);
+/* One step of every row's model, on a pool handle (n <= max_rows, obs_ld >= 965).  First the draw: every row with d_done[i] != 0
+ * (d_done nullable: no draws) gets d_model[i] = the smallest k with r < t_k, r = word x of Philox4x32-10 with counter (low 32 bits
+ * of row_gid0 + i, 65, `counter` lo, `counter` hi) and key (`seed` lo, `seed` hi) (q = 65: apart from the Gumbel draws q = 0..63 and
+ * the heading q = 64 of the training entries).  d_model (int32[n], device) is the caller's and is read by every call: rows keep their
+ * model until they draw.  d_model_rec[i * rec_ld] (nullable) receives (float)d_model[i], or -1 outside [0, K), on every call.
+ * Then, as llq_hier_policy_forward with model d_model[i] for row i: d_state [n, 128], d_actions [n, 12], d_codes, d_heading (both
+ * nullable); a drawn row has d_done[i] != 0, so its state starts from zero.  A row whose model lies outside [0, K) is left untouched. */
+int llq_hier_policy_forward_pool(llq_hier_policy_handle h, const float* d_obs, int64_t obs_ld, int32_t n, const uint8_t* d_done, float* d_state,
+                                 float* d_actions, int32_t* d_codes, float* d_heading, int32_t* d_model, float* d_model_rec, int64_t rec_ld,
+                                 uint64_t seed, uint64_t counter, int64_t row_gid0, void* stream);
 const char* llq_hier_policy_last_error(void);
 
 #ifdef __cplusplus

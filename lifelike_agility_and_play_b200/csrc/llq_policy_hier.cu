@@ -22,6 +22,7 @@
 // step is set.
 #include <cuda_runtime.h>
 
+#include <cmath>
 #include <cstdint>
 #include <string>
 #include <vector>
@@ -224,14 +225,15 @@ __device__ void layer_norm(float* v, int ld, int n, const float* beta, const flo
   __syncthreads();
 }
 // one step of the layer-norm LSTM (nh = 32) for every row: x [kRows][256] in shared memory, state [c(32), h(32)] per row in global memory
-// (updated in place; rows with live[r] == 0 are not stored); arrays lstm + 0..8 = wx, wh, b, beta_x, gamma_x, beta_h, gamma_h, beta_c,
-// gamma_c.  Leaves h in hout[kRows][32].
-__device__ void lstm_step(const Net& n, int lstm, const float* x, float* state, int state_ld, const int* live, const int* wipe, float* zx, float* zh,
-                          float* cbuf, float* hout, float* scratch) {
+// (updated in place; rows with live[r] == 0 are not stored; row r's state is state + rows.srow(r) * state_ld, see BlockRows); arrays
+// lstm + 0..8 = wx, wh, b, beta_x, gamma_x, beta_h, gamma_h, beta_c, gamma_c.  Leaves h in hout[kRows][32].
+template <class Rows>
+__device__ void lstm_step(const Net& n, int lstm, const float* x, float* state, int state_ld, const Rows& rows, const int* live, const int* wipe,
+                          float* zx, float* zh, float* cbuf, float* hout, float* scratch) {
   const int t = threadIdx.x;
   for (int idx = t; idx < kRows * 64; idx += kThreads) {
     const int r = idx >> 6, i = idx & 63;
-    cbuf[idx] = (live[r] && !wipe[r]) ? state[(size_t)r * state_ld + i] : 0.f;          // cbuf[r][0..32) = c, [32..64) = h
+    cbuf[idx] = (live[r] && !wipe[r]) ? state[(size_t)rows.srow(r) * state_ld + i] : 0.f;          // cbuf[r][0..32) = c, [32..64) = h
   }
   __syncthreads();
   dense(x, 256, 256, arr(n, lstm), nullptr, 128, zx, 128, scratch, false);
@@ -249,14 +251,14 @@ __device__ void lstm_step(const Net& n, int lstm, const float* x, float* state, 
     cbuf[r * 64 + u] = c;
     px[u] = c;                                               // layer norm of the new cell state (32 values)
     ph[u] = 1.0f / (1.0f + expf(-go));
-    if (live[r]) state[(size_t)r * state_ld + u] = c;
+    if (live[r]) state[(size_t)rows.srow(r) * state_ld + u] = c;
   }
   __syncthreads();
   layer_norm(zx, 128, 32, arr(n, lstm + 7), arr(n, lstm + 8));
   {
     const float h = zh[r * 128 + u] * tanhf(zx[r * 128 + u]);
     hout[r * 32 + u] = h;
-    if (live[r]) state[(size_t)r * state_ld + 32 + u] = h;
+    if (live[r]) state[(size_t)rows.srow(r) * state_ld + 32 + u] = h;
   }
   __syncthreads();
 }
@@ -302,24 +304,41 @@ __device__ __forceinline__ void game_vector(Smem& S) {
   __syncthreads();
 }
 
-template <int MODE>
-__global__ void __launch_bounds__(kThreads) hier_policy_kernel(Net net, int strategic, const float* __restrict__ obs, long long obs_ld, int n_rows,
-                                                               const unsigned char* __restrict__ done, float* __restrict__ state, float* __restrict__ actions,
-                                                               int* __restrict__ codes, float* __restrict__ heading, Sample smp) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  Smem& S = *reinterpret_cast<Smem*>(smem_raw);
-  const int row0 = blockIdx.x * kRows, t = threadIdx.x;
+// The rows of a CTA.  BlockRows: rows row0 .. row0 + 7 of the batch (hier_policy_kernel).  ListRows: the entries of a pool segment
+// (hier_pool_kernel), row ids in shared memory, -1 for a pad entry.  row(r) indexes the batch (observation, done, outputs); the state of
+// row r is at state + (base() + srow(r)) * ssz.
+struct BlockRows {
+  int row0, n;
+  __device__ __forceinline__ bool live(int r) const { return row0 + r < n; }
+  __device__ __forceinline__ int row(int r) const { return row0 + r; }
+  __device__ __forceinline__ int srow(int r) const { return r; }
+  __device__ __forceinline__ int base() const { return row0; }
+};
+struct ListRows {
+  const int* id;
+  __device__ __forceinline__ bool live(int r) const { return id[r] >= 0; }
+  __device__ __forceinline__ int row(int r) const { return id[r]; }
+  __device__ __forceinline__ int srow(int r) const { return id[r]; }
+  __device__ __forceinline__ int base() const { return 0; }
+};
+
+// The policy forward of one CTA's rows.  The training modes run on BlockRows only (their noise is keyed by rows.row0).
+template <int MODE, class Rows>
+__device__ __forceinline__ void policy_rows(Smem& S, const Rows& rows, Net net, int strategic, const float* __restrict__ obs, long long obs_ld,
+                                            const unsigned char* __restrict__ done, float* __restrict__ state, float* __restrict__ actions,
+                                            int* __restrict__ codes, float* __restrict__ heading, const Sample& smp) {
+  const int t = threadIdx.x;
   if constexpr (MODE == M_TRAIN) strategic = 0;
   if constexpr (MODE == M_TRAIN_SEPMC) strategic = 1;
   const int ow = strategic ? 965 : 916;
   if (t < kRows) {
-    const int live = row0 + t < n_rows;
+    const int live = rows.live(t);
     S.live[t] = live;
-    S.wipe[t] = live && done != nullptr && done[row0 + t] != 0;
+    S.wipe[t] = live && done != nullptr && done[rows.row(t)] != 0;
   }
   for (int idx = t; idx < kRows * kObsLd; idx += kThreads) {
     const int r = idx / kObsLd, i = idx - r * kObsLd;
-    S.obs[r][i] = (row0 + r < n_rows && i < ow) ? obs[(size_t)(row0 + r) * obs_ld + i] : 0.f;
+    S.obs[r][i] = (rows.live(r) && i < ow) ? obs[(size_t)rows.row(r) * obs_ld + i] : 0.f;
   }
   __syncthreads();
   for (int idx = t; idx < kRows * 135; idx += kThreads) {
@@ -328,7 +347,7 @@ __global__ void __launch_bounds__(kThreads) hier_policy_kernel(Net net, int stra
   }
   __syncthreads();
   const int ssz = MODE == M_TRAIN_SEPMC ? 192 : ((MODE == M_TRAIN || strategic) ? 128 : 64);
-  float* st = state + (size_t)row0 * ssz;
+  float* st = state + (size_t)rows.base() * ssz;
   if (strategic) {
     // ---- heading controller
     dense(&S.p[0][0], 136, 135, arr(net, R_HPROP_W), arr(net, R_HPROP_B), 64, &S.cat[0][0], 256, S.scr, true);              // cat[0..64)
@@ -338,26 +357,26 @@ __global__ void __launch_bounds__(kThreads) hier_policy_kernel(Net net, int stra
     dense(&S.x[0][0], 256, 29, arr(net, R_HVEC), arr(net, R_HVEC + 1), 64, &S.y[0][0], 256, S.scr, true);
     dense(&S.y[0][0], 256, 64, arr(net, R_HVEC + 2), arr(net, R_HVEC + 3), 64, &S.cat[0][128], 256, S.scr, true);           // cat[128..192)
     dense(&S.cat[0][0], 256, 192, arr(net, R_HEMB_W), arr(net, R_HEMB_B), 256, &S.x[0][0], 256, S.scr, true);
-    lstm_step(net, R_HLSTM, &S.x[0][0], st, ssz, S.live, S.wipe, &S.zx[0][0], &S.zh[0][0], &S.c[0][0], &S.h[0][0], S.scr);
+    lstm_step(net, R_HLSTM, &S.x[0][0], st, ssz, rows, S.live, S.wipe, &S.zx[0][0], &S.zh[0][0], &S.c[0][0], &S.h[0][0], S.scr);
     if (t < kRows) {
       float a = arr(net, R_HMU_B)[0];
       for (int k = 0; k < 32; k++) a = fmaf(S.h[t][k], arr(net, R_HMU_W)[k], a);
       if constexpr (MODE == M_TRAIN_SEPMC) {
         // heading sample a = mu + exp(logstd) eps: eps from Philox keyed (global row, q = 64, counter) / seed (q 0..63 are the Gumbel draws'
         // of the environmental level); the record gets the raw a and -log p of the raw a, the code controller the clipped one
-        const uint4 r = philox4x32(make_uint4((uint32_t)(smp.row_gid0 + row0 + t), 64u, (uint32_t)smp.counter, (uint32_t)(smp.counter >> 32)),
+        const uint4 r = philox4x32(make_uint4((uint32_t)(smp.row_gid0 + rows.row0 + t), 64u, (uint32_t)smp.counter, (uint32_t)(smp.counter >> 32)),
                                    make_uint2((uint32_t)smp.seed, (uint32_t)(smp.seed >> 32)));
         const float eps = box_muller(r.x, r.y).x, ls = arr(net, RV + SV_LOGSTD)[0];
         a = fmaf(expf(ls), eps, a);
         if (S.live[t]) {
-          if (heading) heading[(size_t)(row0 + t) * smp.out_ld] = a;
-          if (smp.neglogp) smp.neglogp[(size_t)(row0 + t) * smp.out_ld] = 0.5f * eps * eps + ls + 0.91893853320467274f;   // + 0.5 log(2 pi)
+          if (heading) heading[(size_t)(rows.row0 + t) * smp.out_ld] = a;
+          if (smp.neglogp) smp.neglogp[(size_t)(rows.row0 + t) * smp.out_ld] = 0.5f * eps * eps + ls + 0.91893853320467274f;   // + 0.5 log(2 pi)
         }
         S.ang[t] = fminf(fmaxf(a, -3.14159265358979f), 3.14159265358979f);
       } else {
         a = fminf(fmaxf(a, -3.14159265358979f), 3.14159265358979f);
         S.ang[t] = a;
-        if (heading && S.live[t]) heading[row0 + t] = a;
+        if (heading && S.live[t]) heading[rows.row(t)] = a;
       }
     }
     __syncthreads();
@@ -377,11 +396,11 @@ __global__ void __launch_bounds__(kThreads) hier_policy_kernel(Net net, int stra
     dense(&S.x[0][0], 256, 120, arr(net, RV + V_ENC + 26), arr(net, RV + V_ENC + 27), 64, &S.y[0][0], 256, S.scr, true);     // y[0..64)
     dense(&S.y[0][0], 256, 64, arr(net, RV + V_CMD_W), arr(net, RV + V_CMD_B), 128, &S.cat[0][128], 256, S.scr, true);       // cat[128..256)
     dense(&S.cat[0][0], 256, 256, arr(net, RV + V_FC3_W), arr(net, RV + V_FC3_B), 256, &S.x[0][0], 256, S.scr, true);
-    lstm_step(net, RV + V_LSTM, &S.x[0][0], st + 64, ssz, S.live, S.wipe, &S.zx[0][0], &S.zh[0][0], &S.c[0][0], &S.h[0][0], S.scr);
+    lstm_step(net, RV + V_LSTM, &S.x[0][0], st + 64, ssz, rows, S.live, S.wipe, &S.zx[0][0], &S.zh[0][0], &S.c[0][0], &S.h[0][0], S.scr);
     if (t < kRows) {
       float v = arr(net, RV + V_OUT_B)[0];
       for (int k = 0; k < 32; k++) v = fmaf(S.h[t][k], arr(net, RV + V_OUT_W)[k], v);
-      if (smp.values && S.live[t]) smp.values[(size_t)(row0 + t) * smp.out_ld] = v;
+      if (smp.values && S.live[t]) smp.values[(size_t)(rows.row0 + t) * smp.out_ld] = v;
     }
     __syncthreads();
   }
@@ -399,11 +418,11 @@ __global__ void __launch_bounds__(kThreads) hier_policy_kernel(Net net, int stra
     dense(&S.x[0][0], 256, 64, arr(net, RV + SV_GAME + 4), arr(net, RV + SV_GAME + 5), 128, &S.y[0][0], 256, S.scr, true);   // y[0..128)
     dense(&S.cat[0][0], 256, 256, arr(net, RV + SV_CAT_W), arr(net, RV + SV_CAT_B), 256, &S.x[0][0], 256, S.scr, false);     // rows 0-255
     dense<true>(&S.y[0][0], 256, 128, arr(net, RV + SV_CAT_W) + 256 * 256, nullptr, 256, &S.x[0][0], 256, S.scr, true);    // rows 256-383
-    lstm_step(net, RV + SV_LSTM, &S.x[0][0], st + 64, ssz, S.live, S.wipe, &S.zx[0][0], &S.zh[0][0], &S.c[0][0], &S.h[0][0], S.scr);
+    lstm_step(net, RV + SV_LSTM, &S.x[0][0], st + 64, ssz, rows, S.live, S.wipe, &S.zx[0][0], &S.zh[0][0], &S.c[0][0], &S.h[0][0], S.scr);
     if (t < kRows) {
       float v = arr(net, RV + SV_OUT_B)[0];
       for (int k = 0; k < 32; k++) v = fmaf(S.h[t][k], arr(net, RV + SV_OUT_W)[k], v);
-      if (smp.values && S.live[t]) smp.values[(size_t)(row0 + t) * smp.out_ld] = v;
+      if (smp.values && S.live[t]) smp.values[(size_t)(rows.row0 + t) * smp.out_ld] = v;
     }
     __syncthreads();
   }
@@ -418,13 +437,13 @@ __global__ void __launch_bounds__(kThreads) hier_policy_kernel(Net net, int stra
   perception(net, R_MENC, &S.obs[0][0], kObsLd, S.a, S.b, &S.x[0][32], 256);                                                // x[32..120)
   dense(&S.x[0][0], 256, 120, arr(net, R_MENC + 26), arr(net, R_MENC + 27), 64, &S.cat[0][64], 256, S.scr, true);           // cat[64..128)
   dense(&S.cat[0][0], 256, 128, arr(net, R_MEMB_W), arr(net, R_MEMB_B), 256, &S.x[0][0], 256, S.scr, true);
-  lstm_step(net, R_MLSTM, &S.x[0][0], st, ssz, S.live, S.wipe, &S.zx[0][0], &S.zh[0][0], &S.c[0][0], &S.h[0][0], S.scr);
+  lstm_step(net, R_MLSTM, &S.x[0][0], st, ssz, rows, S.live, S.wipe, &S.zx[0][0], &S.zh[0][0], &S.c[0][0], &S.h[0][0], S.scr);
   dense(&S.h[0][0], 32, 32, arr(net, R_LOGIT_W), arr(net, R_LOGIT_B), 256, &S.y[0][0], 256, S.scr, false);                  // logits
   if constexpr (MODE == M_TRAIN) {
     // Gumbel-max sample: code = argmax_j (logit_j + g_j), g from Philox keyed (global row, q, counter) / seed, one call per four logits
     for (int idx = t; idx < kRows * 64; idx += kThreads) {
       const int r = idx >> 6, q = idx & 63;
-      const uint4 b = philox4x32(make_uint4((uint32_t)(smp.row_gid0 + row0 + r), (uint32_t)q, (uint32_t)smp.counter, (uint32_t)(smp.counter >> 32)),
+      const uint4 b = philox4x32(make_uint4((uint32_t)(smp.row_gid0 + rows.row0 + r), (uint32_t)q, (uint32_t)smp.counter, (uint32_t)(smp.counter >> 32)),
                                  make_uint2((uint32_t)smp.seed, (uint32_t)(smp.seed >> 32)));
       *reinterpret_cast<float4*>(&S.x[r][4 * q]) = make_float4(gumbel(b.x), gumbel(b.y), gumbel(b.z), gumbel(b.w));
     }
@@ -448,8 +467,8 @@ __global__ void __launch_bounds__(kThreads) hier_policy_kernel(Net net, int stra
     if (l == 0) {
       S.code[r] = bi;
       if (S.live[r]) {
-        if (codes) codes[row0 + r] = bi;
-        if (smp.neglogp) smp.neglogp[(size_t)(row0 + r) * smp.out_ld] = (m - S.y[r][bi]) + logf(se);
+        if (codes) codes[rows.row0 + r] = bi;
+        if (smp.neglogp) smp.neglogp[(size_t)(rows.row0 + r) * smp.out_ld] = (m - S.y[r][bi]) + logf(se);
       }
     }
   } else {                                                  // argmax per row (warp r), first occurrence
@@ -461,7 +480,7 @@ __global__ void __launch_bounds__(kThreads) hier_policy_kernel(Net net, int stra
       const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
       if (ob > best || (ob == best && oi < bi)) { best = ob; bi = oi; }
     }
-    if (l == 0) { S.code[r] = bi; if (codes && S.live[r]) codes[row0 + r] = bi; }
+    if (l == 0) { S.code[r] = bi; if (codes && S.live[r]) codes[rows.row(r)] = bi; }
   }
   __syncthreads();
   // ---- frozen primitive-level decoder
@@ -474,8 +493,97 @@ __global__ void __launch_bounds__(kThreads) hier_policy_kernel(Net net, int stra
   dense(&S.y[0][0], 256, 256, arr(net, R_LLC + 8), arr(net, R_LLC + 9), 12, &S.x[0][0], 256, S.scr, false);
   if (t < kRows * 12) {
     const int r = t / 12, i = t - 12 * r;
-    if (S.live[r]) actions[(size_t)(row0 + r) * 12 + i] = S.x[r][i];
+    if (S.live[r]) actions[(size_t)rows.row(r) * 12 + i] = S.x[r][i];
   }
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(kThreads) hier_policy_kernel(Net net, int strategic, const float* __restrict__ obs, long long obs_ld, int n_rows,
+                                                               const unsigned char* __restrict__ done, float* __restrict__ state, float* __restrict__ actions,
+                                                               int* __restrict__ codes, float* __restrict__ heading, Sample smp) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  policy_rows<MODE>(*reinterpret_cast<Smem*>(smem_raw), BlockRows{(int)blockIdx.x * kRows, n_rows}, net, strategic, obs, obs_ld, done, state, actions,
+                    codes, heading, smp);
+}
+
+// ---- opponent pool (llq_hier_policy_forward_pool): K deterministic strategic-level models, every row run with its own model
+constexpr int kAssignThreads = 1024;
+// model k is drawn for r < t[k] (and r >= t[k - 1]); t[K - 1] = 2^32; by value, so a new table takes effect at the next launch
+struct Cutoffs { unsigned long long t[LLQ_HIER_POOL_MAX]; };
+// the pool kernel's shared memory: Smem, then the row ids of the CTA's segment entries
+struct PoolSmem : Smem { int rid[kRows]; };
+
+// One CTA.  Draws a model for every row with done[i] != 0 (r = word x of Philox4x32-10, counter (low 32 bits of row_gid0 + i, 65,
+// counter lo, counter hi), key (seed lo, seed hi); model = the smallest k with r < t[k]), records every row's model (-1 outside
+// [0, K)), and buckets the rows by model: segment k holds its rows in ascending order, padded with -1 to a multiple of kRows, and
+// starts at CTA seg_cta[k] of the pool forward (seg_cta[K] = the CTAs of all segments); its entries are seg_rows[seg_cta[k] * kRows ..).
+__global__ void __launch_bounds__(kAssignThreads) hier_pool_assign_kernel(int n, int n_models, Cutoffs cut, const unsigned char* __restrict__ done,
+                                                                          int* __restrict__ model, float* __restrict__ rec, long long rec_ld,
+                                                                          unsigned long long seed, unsigned long long counter, long long row_gid0,
+                                                                          int* __restrict__ seg_cta, int* __restrict__ seg_rows) {
+  __shared__ int cnt[LLQ_HIER_POOL_MAX], first[LLQ_HIER_POOL_MAX], fill[LLQ_HIER_POOL_MAX];
+  __shared__ int chunk[kAssignThreads];
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  if (t < LLQ_HIER_POOL_MAX) { cnt[t] = 0; fill[t] = 0; }
+  __syncthreads();
+  for (int i = t; i < n; i += kAssignThreads) {
+    int m = model[i];
+    if (done != nullptr && done[i] != 0) {
+      const uint32_t r = philox4x32(make_uint4((uint32_t)(row_gid0 + i), 65u, (uint32_t)counter, (uint32_t)(counter >> 32)),
+                                    make_uint2((uint32_t)seed, (uint32_t)(seed >> 32))).x;
+      m = 0;                                                 // the cutoffs do not decrease: the count of t[k] <= r is the smallest k with r < t[k]
+#pragma unroll
+      for (int k = 0; k < LLQ_HIER_POOL_MAX - 1; k++) m += (k < n_models - 1 && (unsigned long long)r >= cut.t[k]) ? 1 : 0;
+      model[i] = m;
+    }
+    const bool in = m >= 0 && m < n_models;
+    if (rec != nullptr) rec[(size_t)i * rec_ld] = in ? (float)m : -1.f;
+    if (in) atomicAdd(&cnt[m], 1);
+  }
+  __syncthreads();
+  if (t == 0) {
+    int c = 0;
+    for (int k = 0; k < n_models; k++) { first[k] = c; seg_cta[k] = c; c += (cnt[k] + kRows - 1) / kRows; }
+    seg_cta[n_models] = c;
+  }
+  __syncthreads();
+  // stable placement, kAssignThreads rows at a time: warp w places the rows of models w, w + 32 in ascending order (a ballot per 32 rows)
+  for (int c0 = 0; c0 < n; c0 += kAssignThreads) {
+    const int len = min(kAssignThreads, n - c0);
+    chunk[t] = t < len ? model[c0 + t] : -1;                 // thread t wrote model[c0 + t] above: its own write
+    __syncthreads();
+    for (int k = warp; k < n_models; k += kAssignThreads / 32) {
+      int pos = fill[k];
+      for (int s = 0; s < len; s += 32) {
+        const bool mine = chunk[s + lane] == k;
+        const unsigned bal = __ballot_sync(0xffffffffu, mine);
+        if (mine) seg_rows[first[k] * kRows + pos + __popc(bal & ((1u << lane) - 1u))] = c0 + s + lane;
+        pos += __popc(bal);
+      }
+      if (lane == 0) fill[k] = pos;
+    }
+    __syncthreads();
+  }
+  if (t < n_models)
+    for (int j = cnt[t]; j % kRows; j++) seg_rows[first[t] * kRows + j] = -1;
+}
+
+// The deterministic strategic-level forward of a pool: CTA b runs the kRows entries seg_rows[b * kRows ..) of its segment k (the largest
+// k with seg_cta[k] <= b) with model k, whose offset table is off + k * RV; CTAs from seg_cta[K] on return at once.
+__global__ void __launch_bounds__(kThreads) hier_pool_kernel(const float* __restrict__ w, const int* __restrict__ off, int n_models,
+                                                             const int* __restrict__ seg_cta, const int* __restrict__ seg_rows,
+                                                             const float* __restrict__ obs, long long obs_ld, const unsigned char* __restrict__ done,
+                                                             float* __restrict__ state, float* __restrict__ actions, int* __restrict__ codes,
+                                                             float* __restrict__ heading) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  PoolSmem& S = *reinterpret_cast<PoolSmem*>(smem_raw);
+  const int b = blockIdx.x;
+  if (b >= seg_cta[n_models]) return;
+  int k = 0;
+  for (int j = 1; j < n_models; j++) if (seg_cta[j] <= b) k = j;
+  if (threadIdx.x < kRows) S.rid[threadIdx.x] = seg_rows[b * kRows + threadIdx.x];
+  __syncthreads();
+  policy_rows<M_DET>(S, ListRows{S.rid}, Net{w, off + k * RV}, 1, obs, obs_ld, done, state, actions, codes, heading, Sample{});
 }
 
 }  // namespace
@@ -485,9 +593,33 @@ struct llq_hier_policy {
   bool attr_set = false;
   float* d_w = nullptr;
   int* d_off = nullptr;
+  // pool handles (llq_hier_policy_create_pool): K models, the cutoffs of the next draws, the assign kernel's workspace
+  int n_models = 0, max_rows = 0;
+  Cutoffs cut{};
+  int* d_seg = nullptr;                                      // [K + 1] first CTA of every segment, then the segments' row ids
 };
 
 namespace {
+
+// the device checks and the upload of the blob and of the device offset table `off`, once the arguments are checked
+int upload(const float* weights, int64_t n_weights, const std::vector<int>& off, int32_t strategic, int train, int32_t device,
+           llq_hier_policy_handle* out) {
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail_h(LLQ_ECUDA, "no CUDA device visible (no CPU fallback)");
+  if (device < 0 || device >= ndev) return fail_h(LLQ_EINVAL, "device ordinal out of range");
+  if (cudaSetDevice(device) != cudaSuccess) return fail_h(LLQ_ECUDA, "cudaSetDevice failed");
+  llq_hier_policy* h = new (std::nothrow) llq_hier_policy();
+  if (!h) return fail_h(LLQ_ENOMEM, "out of memory");
+  h->device = device; h->strategic = strategic ? 1 : 0; h->train = train;
+  if (cudaMalloc(&h->d_w, sizeof(float) * (size_t)n_weights) != cudaSuccess || cudaMalloc(&h->d_off, sizeof(int) * off.size()) != cudaSuccess ||
+      cudaMemcpy(h->d_w, weights, sizeof(float) * (size_t)n_weights, cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy(h->d_off, off.data(), sizeof(int) * off.size(), cudaMemcpyHostToDevice) != cudaSuccess) {
+    cudaFree(h->d_w); cudaFree(h->d_off); delete h;
+    return fail_h(LLQ_ECUDA, "weight upload failed");
+  }
+  *out = h;
+  return LLQ_OK;
+}
 
 // `value_offsets` (n_value entries: LLQ_HIER_ROLES_VALUE, or LLQ_HIER_ROLES_TRAIN_STRATEGIC at the strategic level) null: a deterministic
 // handle
@@ -499,24 +631,20 @@ int create(const float* weights, int64_t n_weights, const int32_t* offsets, int3
   if (value_offsets)
     for (int i = 0; i < n_value; i++)
       if (value_offsets[i] < 0 || value_offsets[i] >= n_weights) return fail_h(LLQ_EINVAL, "training-table offset outside the weight blob");
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail_h(LLQ_ECUDA, "no CUDA device visible (no CPU fallback)");
-  if (device < 0 || device >= ndev) return fail_h(LLQ_EINVAL, "device ordinal out of range");
-  if (cudaSetDevice(device) != cudaSuccess) return fail_h(LLQ_ECUDA, "cudaSetDevice failed");
-  llq_hier_policy* h = new (std::nothrow) llq_hier_policy();
-  if (!h) return fail_h(LLQ_ENOMEM, "out of memory");
-  h->device = device; h->strategic = strategic ? 1 : 0; h->train = value_offsets ? 1 : 0;
   std::vector<int> off(RV + kTrainRoles, 0);
   for (int i = 0; i < n_roles; i++) off[i] = offsets[i];
   if (value_offsets) for (int i = 0; i < n_value; i++) off[RV + i] = value_offsets[i];
-  if (cudaMalloc(&h->d_w, sizeof(float) * (size_t)n_weights) != cudaSuccess || cudaMalloc(&h->d_off, sizeof(int) * off.size()) != cudaSuccess ||
-      cudaMemcpy(h->d_w, weights, sizeof(float) * (size_t)n_weights, cudaMemcpyHostToDevice) != cudaSuccess ||
-      cudaMemcpy(h->d_off, off.data(), sizeof(int) * off.size(), cudaMemcpyHostToDevice) != cudaSuccess) {
-    cudaFree(h->d_w); cudaFree(h->d_off); delete h;
-    return fail_h(LLQ_ECUDA, "weight upload failed");
-  }
-  *out = h;
-  return LLQ_OK;
+  return upload(weights, n_weights, off, strategic, value_offsets ? 1 : 0, device, out);
+}
+
+// the cutoffs of probs[0..K) (checked by the caller): sequential fp64 sums, t_k = floor(cum_k / cum_{K-1} 2^32), t_{K-1} = 2^32
+Cutoffs cutoffs(const double* probs, int K) {
+  Cutoffs c{};
+  double cum[LLQ_HIER_POOL_MAX], s = 0.0;
+  for (int k = 0; k < K; k++) { s += probs[k]; cum[k] = s; }
+  for (int k = 0; k < K - 1; k++) c.t[k] = (unsigned long long)std::floor(cum[k] / s * 4294967296.0);
+  c.t[K - 1] = 1ull << 32;
+  return c;
 }
 
 template <int MODE>
@@ -566,7 +694,7 @@ int llq_hier_policy_create_train_strategic(const float* weights, int64_t n_weigh
 int llq_hier_policy_destroy(llq_hier_policy_handle h) {
   if (!h) return LLQ_OK;
   cudaSetDevice(h->device);
-  cudaFree(h->d_w); cudaFree(h->d_off);
+  cudaFree(h->d_w); cudaFree(h->d_off); cudaFree(h->d_seg);
   delete h;
   return LLQ_OK;
 }
@@ -574,6 +702,7 @@ int llq_hier_policy_destroy(llq_hier_policy_handle h) {
 int llq_hier_policy_forward(llq_hier_policy_handle h, const float* d_obs, int64_t obs_ld, int32_t n, const uint8_t* d_done, float* d_state,
                             float* d_actions, int32_t* d_codes, float* d_heading, void* stream) {
   if (!h || !d_obs || !d_state || !d_actions) return fail_h(LLQ_EINVAL, "null argument");
+  if (h->n_models) return fail_h(LLQ_EINVAL, "a pool handle steps with llq_hier_policy_forward_pool");
   if (h->train)
     return fail_h(LLQ_EINVAL, h->strategic ? "a strategic training handle steps with llq_hier_policy_forward_rec_strategic (its state rows are 192 floats)"
                                            : "a training handle steps with llq_hier_policy_forward_rec (its state rows are 128 floats)");
@@ -600,6 +729,73 @@ int llq_hier_policy_forward_rec_strategic(llq_hier_policy_handle h, const float*
   if (n <= 0 || obs_ld < 965 || out_ld < 1) return fail_h(LLQ_EINVAL, "bad row count or row stride");
   const Sample smp{d_values, d_neglogp, (long long)out_ld, (unsigned long long)seed, (unsigned long long)counter, (long long)row_gid0};
   return launch<M_TRAIN_SEPMC>(h, d_obs, obs_ld, n, d_done, d_state, d_actions, d_codes, d_heading, smp, stream);
+}
+
+int llq_hier_policy_create_pool(const float* weights, int64_t n_weights, const int32_t* offsets, int32_t n_models, int32_t max_rows, int32_t device,
+                                llq_hier_policy_handle* out) {
+  if (!weights || !offsets || !out) return fail_h(LLQ_EINVAL, "null argument");
+  if (n_models < 1 || n_models > LLQ_HIER_POOL_MAX) return fail_h(LLQ_EINVAL, "n_models outside [1, LLQ_HIER_POOL_MAX]");
+  if (max_rows <= 0) return fail_h(LLQ_EINVAL, "max_rows must be positive");
+  std::vector<int> off((size_t)n_models * RV);
+  for (size_t i = 0; i < off.size(); i++) {
+    if (offsets[i] < 0 || offsets[i] >= n_weights) return fail_h(LLQ_EINVAL, "role offset outside the weight blob");
+    off[i] = offsets[i];
+  }
+  llq_hier_policy_handle h = nullptr;
+  const int rc = upload(weights, n_weights, off, 1, 0, device, &h);
+  if (rc != LLQ_OK) return rc;
+  h->n_models = n_models; h->max_rows = max_rows;
+  const std::vector<double> uniform(n_models, 1.0);
+  h->cut = cutoffs(uniform.data(), n_models);
+  const size_t ws = (size_t)n_models + 1 + ((size_t)(max_rows + kRows - 1) / kRows + n_models) * kRows;
+  if (cudaMalloc(&h->d_seg, sizeof(int) * ws) != cudaSuccess) {
+    llq_hier_policy_destroy(h);
+    return fail_h(LLQ_ECUDA, "workspace allocation failed");
+  }
+  *out = h;
+  return LLQ_OK;
+}
+
+int llq_hier_policy_set_pool_probs(llq_hier_policy_handle h, const double* probs, int32_t n) {
+  if (!h || !probs) return fail_h(LLQ_EINVAL, "null argument");
+  if (!h->n_models) return fail_h(LLQ_EINVAL, "not a pool handle (llq_hier_policy_create_pool)");
+  if (n != h->n_models) return fail_h(LLQ_EINVAL, "one probability per model");
+  double s = 0.0;
+  for (int k = 0; k < n; k++) {
+    if (!std::isfinite(probs[k]) || probs[k] < 0.0) return fail_h(LLQ_EINVAL, "probabilities must be finite and >= 0");
+    s += probs[k];
+  }
+  if (!(s > 0.0) || !std::isfinite(s)) return fail_h(LLQ_EINVAL, "probabilities must have a finite positive sum");
+  h->cut = cutoffs(probs, n);
+  return LLQ_OK;
+}
+
+int llq_hier_policy_forward_pool(llq_hier_policy_handle h, const float* d_obs, int64_t obs_ld, int32_t n, const uint8_t* d_done, float* d_state,
+                                 float* d_actions, int32_t* d_codes, float* d_heading, int32_t* d_model, float* d_model_rec, int64_t rec_ld,
+                                 uint64_t seed, uint64_t counter, int64_t row_gid0, void* stream) {
+  if (!h || !d_obs || !d_state || !d_actions || !d_model) return fail_h(LLQ_EINVAL, "null argument");
+  if (!h->n_models) return fail_h(LLQ_EINVAL, "not a pool handle (llq_hier_policy_create_pool)");
+  if (n <= 0 || n > h->max_rows) return fail_h(LLQ_EINVAL, "row count outside [1, max_rows]");
+  if (obs_ld < 965 || (d_model_rec && rec_ld < 1)) return fail_h(LLQ_EINVAL, "bad row stride");
+  if (cudaSetDevice(h->device) != cudaSuccess) return fail_h(LLQ_ECUDA, "cudaSetDevice failed");
+  if (!h->attr_set) {
+    if (cudaFuncSetAttribute(hier_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(PoolSmem)) != cudaSuccess)
+      return fail_h(LLQ_ECUDA, "cudaFuncSetAttribute failed");
+    h->attr_set = true;
+  }
+  const int K = h->n_models;
+  int* seg_cta = h->d_seg;
+  int* seg_rows = h->d_seg + K + 1;
+  hier_pool_assign_kernel<<<1, kAssignThreads, 0, (cudaStream_t)stream>>>(n, K, h->cut, d_done, d_model, d_model_rec, (long long)rec_ld,
+                                                                         (unsigned long long)seed, (unsigned long long)counter, (long long)row_gid0,
+                                                                         seg_cta, seg_rows);
+  if (cudaGetLastError() != cudaSuccess) return fail_h(LLQ_ECUDA, "hier_pool_assign_kernel launch failed");
+  // every segment ends within kRows - 1 pad entries: at most ceil(n / kRows) + K - 1 CTAs, fixed here without reading the segments back
+  hier_pool_kernel<<<(n + kRows - 1) / kRows + K, kThreads, sizeof(PoolSmem), (cudaStream_t)stream>>>(h->d_w, h->d_off, K, seg_cta, seg_rows, d_obs,
+                                                                                                      obs_ld, d_done, d_state, d_actions, d_codes,
+                                                                                                      d_heading);
+  if (cudaGetLastError() != cudaSuccess) return fail_h(LLQ_ECUDA, "hier_pool_kernel launch failed");
+  return LLQ_OK;
 }
 
 const char* llq_hier_policy_last_error(void) { return g_err_h.c_str(); }

@@ -5,18 +5,22 @@ learning model against one from the pool; the game's termination reads robot 0's
   * the strategic training forward (llq_hier_policy_forward_rec_strategic) on the seat-0 rows of slab row t, read in place with a row
     stride of two records, samples the heading and writes its raw value, -log p and V straight into those records; its noise is keyed by
     the global pair id;
-  * the opponent's deterministic forward (llq_hier_policy_forward) on the seat-1 rows;
+  * the opponent's deterministic forward (llq_hier_policy_forward) on the seat-1 rows; against an opponent pool
+    (policy_epmc.DeviceOpponentPool, llq_hier_policy_forward_pool) every pair whose game starts first draws its opponent's model from the
+    pool's probabilities, and the model index goes into the opponent column of the pair's seat-0 record;
   * device-side copies interleave both seats' actions into the engine's [2P, 12] action array and put both seats' codes into the code
     column; the fused env step (record option 2) writes a_t | r_t | done_t into row t and observation t+1 into row t+1; the pair's done
     flags (equal on both rows) are copied into each seat's contiguous mask for the next forwards.
-The LSTM states ([P, 192] for seat 0: heading, code and value LSTM; [P, 128] for seat 1) stay on the device.  Nothing synchronises with
+The LSTM states ([P, 192] for seat 0: heading, code and value LSTM; [P, 128] for seat 1) and, with a pool, each pair's model index stay on
+the device.  Nothing synchronises with
 the host inside an unroll.  Two `[T+1, 2P, 984]` slabs ping-pong (layout: parallel/trajectory.py, SCOL_*).
 """
 from collections import namedtuple
 
 import torch
 
-from .trajectory import ACT_DIM, SCOL_CODE, SCOL_HEADING, SCOL_NEGLOGP, SCOL_VALUE, SEPMC_OBS_DIM, SEPMC_TRAJ_WIDTH
+from ..policy_epmc import DeviceOpponentPool
+from .trajectory import ACT_DIM, SCOL_CODE, SCOL_HEADING, SCOL_NEGLOGP, SCOL_OPPONENT, SCOL_VALUE, SEPMC_OBS_DIM, SEPMC_TRAJ_WIDTH
 
 SepmcUnroll = namedtuple("SepmcUnroll", ["slab", "initial_state", "first_mask", "bootstrap_value"])
 _FSZ = 4
@@ -26,7 +30,8 @@ class SepmcRolloutWorker:
     def __init__(self, engine, policy, opponent, unroll, device, seed=0):
         """`engine`: a `_capi.VecEngine` on the CUDA library for the SEPMC env (965-wide observations, 2P robots) with auto_reset=1 and an
         even `global_env_offset`; `policy`: a `policy_epmc.DeviceSepmcTrainPolicy` (the learner's weights); `opponent`: a deterministic
-        strategic-level `policy_epmc.DeviceHierPolicy` (its own weights), both on the engine's device; `unroll`: T."""
+        strategic-level `policy_epmc.DeviceHierPolicy` (its own weights), or a `policy_epmc.DeviceOpponentPool` with max_rows >= P (each
+        pair draws its opponent's model at every game start; see `set_opponent_probs`), all on the engine's device; `unroll`: T."""
         if engine.obs_dim != SEPMC_OBS_DIM:
             raise ValueError("SepmcRolloutWorker drives the SEPMC env (965-wide observations)")
         if not int(engine.cfg.auto_reset):
@@ -36,7 +41,10 @@ class SepmcRolloutWorker:
         if getattr(policy, "state_dim", None) != 192 or not getattr(policy, "train", False):
             raise ValueError("SepmcRolloutWorker needs a DeviceSepmcTrainPolicy")
         if not getattr(opponent, "strategic", False) or getattr(opponent, "train", True):
-            raise ValueError("the opponent must be a deterministic strategic-level DeviceHierPolicy")
+            raise ValueError("the opponent must be a deterministic strategic-level DeviceHierPolicy or a DeviceOpponentPool")
+        self.pool = isinstance(opponent, DeviceOpponentPool)
+        if self.pool and opponent.max_rows < engine.n // 2:
+            raise ValueError("the opponent pool's max_rows is below the number of pairs")
         self.eng, self.pol, self.opp, self.T = engine, policy, opponent, int(unroll)
         self.n, self.P = engine.n, engine.n // 2
         self.dev = torch.device(device)
@@ -50,6 +58,7 @@ class SepmcRolloutWorker:
         self.act, self.rew = z(self.n, ACT_DIM), z(self.n)
         self.seat_act = z(2, P, ACT_DIM)
         self.codes = z(2, P, dtype=torch.int32)
+        self.opp_model = z(P, dtype=torch.int32) if self.pool else None     # each pair's model in the pool, redrawn where masks[1] is set
         # per slab: the state and mask its first forward started from, V(observation T)
         self.init_states = [z(P, policy.state_dim) for _ in range(2)]
         self.first_masks = [z(P, dtype=torch.uint8) for _ in range(2)]
@@ -93,8 +102,13 @@ class SepmcRolloutWorker:
                 self.first_masks[i].copy_(self.masks[0])
             self._forward(row, self.state, self.seat_act[0], p0 + SCOL_HEADING * _FSZ, p0 + SCOL_VALUE * _FSZ, p0 + SCOL_NEGLOGP * _FSZ,
                           self.codes[0].data_ptr(), 2 * SEPMC_TRAJ_WIDTH)
-            self.opp.forward(p1, 2 * SEPMC_TRAJ_WIDTH, self.P, self.masks[1].data_ptr(), self.opp_state.data_ptr(), self.seat_act[1].data_ptr(),
-                             self.codes[1].data_ptr(), None, self.stream.cuda_stream)
+            if self.pool:
+                self.opp.forward(p1, 2 * SEPMC_TRAJ_WIDTH, self.P, self.masks[1].data_ptr(), self.opp_state.data_ptr(), self.seat_act[1].data_ptr(),
+                                 self.codes[1].data_ptr(), None, self.opp_model.data_ptr(), p0 + SCOL_OPPONENT * _FSZ, 2 * SEPMC_TRAJ_WIDTH,
+                                 self.seed, self.calls, self.pair_gid0, self.stream.cuda_stream)
+            else:
+                self.opp.forward(p1, 2 * SEPMC_TRAJ_WIDTH, self.P, self.masks[1].data_ptr(), self.opp_state.data_ptr(),
+                                 self.seat_act[1].data_ptr(), self.codes[1].data_ptr(), None, self.stream.cuda_stream)
             self.act.view(self.P, 2, ACT_DIM).copy_(self.seat_act.transpose(0, 1))
             row[:, SCOL_CODE].view(self.P, 2).copy_(self.codes.t())
         self.eng.step_device(self.act.data_ptr(), nxt.data_ptr(), self.rew.data_ptr(), self.done.data_ptr(), obs_ld=SEPMC_TRAJ_WIDTH,
@@ -120,6 +134,12 @@ class SepmcRolloutWorker:
             self.buf[0, :, :SEPMC_OBS_DIM] = done_buf[self.T, :, :SEPMC_OBS_DIM]
         self.t = 0
         return SepmcUnroll(done_buf[:self.T], self.init_states[idx], self.first_masks[idx], self.boots[idx])
+
+    def set_opponent_probs(self, probs):
+        """The opponent pool's draw probabilities (one per model, >= 0, positive sum) for the games that start from the next step on."""
+        if not self.pool:
+            raise ValueError("the worker plays a single opponent")
+        self.opp.set_probs(probs)
 
     def wait(self):
         """Make torch's current stream wait for everything queued so far (call before reading a finished slab there)."""

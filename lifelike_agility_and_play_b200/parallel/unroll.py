@@ -26,8 +26,8 @@ import numpy as np
 import torch
 
 from .trajectory import (ACT_DIM, COL_ACTION, COL_DONE, COL_NEGLOGP, COL_REWARD, COL_VALUE, HCOL_CODE, HCOL_DONE, HCOL_NEGLOGP, HCOL_REWARD,
-                         HCOL_VALUE, HIER_TRAJ_WIDTH, OBS_DIM, SCOL_CODE, SCOL_DONE, SCOL_HEADING, SCOL_NEGLOGP, SCOL_REWARD, SCOL_VALUE,
-                         SEPMC_TRAJ_WIDTH, TRAJ_WIDTH)
+                         HCOL_VALUE, HIER_TRAJ_WIDTH, OBS_DIM, SCOL_CODE, SCOL_DONE, SCOL_HEADING, SCOL_NEGLOGP, SCOL_OPPONENT, SCOL_REWARD,
+                         SCOL_VALUE, SEPMC_TRAJ_WIDTH, TRAJ_WIDTH)
 
 OBS_LEAVES = OrderedDict([("prop", 99), ("prop_a", 36), ("future", 72)])        # PLE:117-124
 # leaf order of a flattened PMCInputs record (namedtuple order, the observation dict in key-insertion order)
@@ -121,13 +121,14 @@ def _recurrent_records(slab, leaves, done, r, v, first_mask, bootstrap_value, ga
     return out
 
 
-def sepmc_slab_records(slab, initial_state, first_mask, bootstrap_value, gamma=GAMMA, lam=LAM):
+def sepmc_slab_records(slab, initial_state, first_mask, bootstrap_value, gamma=GAMMA, lam=LAM, with_opponent=False):
     """Learner tensors of a strategic-level unroll (`SepmcRolloutWorker.finish_unroll()`) for the learning robot (seat 0: rows 0, 2, 4, ...
     of the `[T, 2P, 984]` slab), on the slab's device, named: the twelve observation leaves [T, P, *leaf] (CTG:111-124), `A_HLC` [T, P]
     (the raw sampled heading), `A_Z` [T, P] int64 (the argmax code), `neglogp` (of the heading), `discount` = gamma (1 - done), `r`, `V`,
     `R` (lambda-returns, bootstrapped with V(observation T)), `M` [T, P] = the mask each forward received (M[0] = first_mask, M[t] =
     done[t-1]) -- all [T, P] float32 but A_Z -- and `S` [P, 192], the recurrent state the unroll started from (heading, code and value
-    LSTM, [c, h] each)."""
+    LSTM, [c, h] each).  `with_opponent`: also `opponent` [T, P] int64 last, the index of the model seat 1 played in an opponent
+    pool (for the league's per-opponent statistics; 0 against a single opponent)."""
     assert slab.dim() == 3 and slab.shape[2] == SEPMC_TRAJ_WIDTH and slab.shape[1] % 2 == 0, \
         "expected a [T, 2P, %d] trajectory slab" % SEPMC_TRAJ_WIDTH
     s0 = slab[:, 0::2]
@@ -139,6 +140,8 @@ def sepmc_slab_records(slab, initial_state, first_mask, bootstrap_value, gamma=G
     head["neglogp"] = s0[:, :, SCOL_NEGLOGP]
     head.update(out)
     head["S"] = initial_state
+    if with_opponent:
+        head["opponent"] = s0[:, :, SCOL_OPPONENT].to(torch.int64)
     return head
 
 

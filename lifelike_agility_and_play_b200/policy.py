@@ -72,7 +72,8 @@ import os as _os
 POLICY_LIB_PATH = _os.path.join(_os.path.dirname(_os.path.abspath(__file__)), "csrc", "libllq_policy.so")
 POLICY_EXPORTS = ["llq_policy_create", "llq_policy_destroy", "llq_policy_forward", "llq_policy_forward_ex", "llq_policy_forward_rec",
                   "llq_policy_last_error", "llq_hier_policy_create", "llq_hier_policy_destroy", "llq_hier_policy_forward",
-                  "llq_hier_policy_last_error", "llq_hier_policy_create_train", "llq_hier_policy_forward_rec"]
+                  "llq_hier_policy_last_error", "llq_hier_policy_create_train", "llq_hier_policy_forward_rec",
+                  "llq_hier_policy_create_pool", "llq_hier_policy_set_pool_probs", "llq_hier_policy_forward_pool"]
 N_WEIGHTS = 358647
 
 

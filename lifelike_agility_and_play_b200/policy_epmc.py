@@ -467,3 +467,60 @@ class DeviceSepmcTrainPolicy(DeviceHierPolicy):
                                                             C.c_void_p(stream or 0))
         if rc:
             raise RuntimeError("llq_hier_policy_forward_rec_strategic: %s" % self.lib.llq_hier_policy_last_error().decode())
+
+
+class DeviceOpponentPool:
+    """K frozen strategic-level models on the GPU in one handle (include/llq_policy.h, llq_hier_policy_create_pool): `forward` draws a
+    new model for every row whose done flag is set, from the probabilities of `set_probs` (uniform until then), and runs every row's
+    deterministic forward with its own model in one launch.  `models`: a list of 1 .. 64 strategic-level models (152 arrays each);
+    `max_rows` bounds the rows of every forward.  Single-owner: the handle holds one workspace, so one stream at a time."""
+
+    def __init__(self, models, device=0, *, max_rows, probs=None):
+        import ctypes as C
+        self._C, self.lib = C, _policy_lib()
+        self._h = None
+        assert all(len(m) == 152 for m in models), "expected strategic-level models (152 arrays)"
+        blobs, offs, base = [], [], 0
+        for m in models:
+            blob, starts = _weight_blob(m)
+            offs.append(np.array([starts[i] for i in hier_role_arrays(True)], np.int64) + base)
+            blobs.append(blob)
+            base += blob.size
+        blob = np.concatenate(blobs) if blobs else np.zeros(0, np.float32)
+        off = np.concatenate(offs).astype(np.int32) if offs else np.zeros(0, np.int32)
+        h = C.c_void_p()
+        rc = self.lib.llq_hier_policy_create_pool(blob.ctypes.data_as(C.c_void_p), C.c_int64(blob.size), off.ctypes.data_as(C.c_void_p),
+                                                  C.c_int32(len(models)), C.c_int32(int(max_rows)), C.c_int32(device), C.byref(h))
+        if rc:
+            raise RuntimeError("llq_hier_policy_create_pool: %s" % self.lib.llq_hier_policy_last_error().decode())
+        self._h = h
+        self.strategic, self.train = True, False
+        self.n_models, self.max_rows = len(models), int(max_rows)
+        self.state_dim, self.obs_dim = 128, 965
+        if probs is not None:
+            self.set_probs(probs)
+
+    def set_probs(self, probs):
+        """Draw probabilities of the next forwards: one finite entry >= 0 per model, positive sum (they need not sum to 1)."""
+        C = self._C
+        p = np.ascontiguousarray(probs, np.float64).reshape(-1)
+        rc = self.lib.llq_hier_policy_set_pool_probs(self._h, p.ctypes.data_as(C.c_void_p), C.c_int32(p.size))
+        if rc:
+            raise ValueError("llq_hier_policy_set_pool_probs: %s" % self.lib.llq_hier_policy_last_error().decode())
+
+    def forward(self, obs_ptr, obs_ld, n, done_ptr, state_ptr, act_ptr, codes_ptr, heading_ptr, model_ptr, model_rec_ptr, rec_ld, seed, counter,
+                row_gid0=0, stream=None):
+        """One step (include/llq_policy.h, llq_hier_policy_forward_pool): rows with done set draw a model into model_ptr (int32[n]), keyed
+        by (row_gid0 + i, counter) and `seed`; model_rec_ptr + i * rec_ld floats (nullable) records every row's model."""
+        C = self._C
+        rc = self.lib.llq_hier_policy_forward_pool(self._h, C.c_void_p(obs_ptr), C.c_int64(obs_ld), C.c_int32(n), C.c_void_p(done_ptr or 0),
+                                                   C.c_void_p(state_ptr), C.c_void_p(act_ptr), C.c_void_p(codes_ptr or 0), C.c_void_p(heading_ptr or 0),
+                                                   C.c_void_p(model_ptr), C.c_void_p(model_rec_ptr or 0), C.c_int64(rec_ld), C.c_uint64(seed),
+                                                   C.c_uint64(counter), C.c_int64(row_gid0), C.c_void_p(stream or 0))
+        if rc:
+            raise RuntimeError("llq_hier_policy_forward_pool: %s" % self.lib.llq_hier_policy_last_error().decode())
+
+    def close(self):
+        if self._h:
+            self.lib.llq_hier_policy_destroy(self._h)
+            self._h = None
