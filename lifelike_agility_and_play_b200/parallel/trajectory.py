@@ -16,15 +16,16 @@ import torch.distributed as dist
 OBS_DIM, ACT_DIM = 207, 12
 COL_ACTION, COL_REWARD, COL_DONE, COL_NEGLOGP, COL_VALUE = 207, 219, 220, 221, 222
 TRAJ_WIDTH = 223
-# the environmental level's record (parallel/hier_rollout.py): obs 916 | action 12 | reward | done (the step kernel, record option 2) |
-# -log p | value | sampled code (as a float), padded to a multiple of 4 floats
+# the environmental level's record (parallel/rollout.py, HierRolloutWorker): obs 916 | action 12 | reward | done (the step kernel, record
+# option 2) | -log p | value | sampled code (as a float), padded to a multiple of 4 floats
 HIER_OBS_DIM = 916
 HCOL_ACTION, HCOL_REWARD, HCOL_DONE, HCOL_NEGLOGP, HCOL_VALUE, HCOL_CODE = 916, 928, 929, 930, 931, 932
 HIER_TRAJ_WIDTH = 936
-# the strategic level's record, one row per robot (parallel/sepmc_rollout.py): obs 965 | action 12 | reward | done (the step kernel, record
-# option 2) | -log p | value | code (as a float) | raw sampled heading | opponent (as a float), 984 floats, a multiple of 4.  The learning
-# robot's rows (seat 0) carry all of them; the frozen opponent's (seat 1) carry the code and leave the rest at 0.  `opponent` is the
-# index of the model seat 1 plays in an opponent pool (policy_epmc.DeviceOpponentPool), and stays 0 against a single opponent.
+# the strategic level's record, one row per robot (parallel/rollout.py, SepmcRolloutWorker): obs 965 | action 12 | reward | done (the
+# step kernel, record option 2) | -log p | value | code (as a float) | raw sampled heading | opponent (as a float), 984 floats, a multiple
+# of 4.  The learning robot's rows (seat 0) carry all of them; the frozen opponent's (seat 1) carry the code and leave the rest at 0.
+# `opponent` is the index of the model seat 1 plays in an opponent pool (policy_epmc.DeviceOpponentPool), and stays 0 against a single
+# opponent.
 SEPMC_OBS_DIM = 965
 SCOL_ACTION, SCOL_REWARD, SCOL_DONE, SCOL_NEGLOGP, SCOL_VALUE, SCOL_CODE, SCOL_HEADING = 965, 977, 978, 979, 980, 981, 982
 SCOL_OPPONENT = 983

@@ -79,6 +79,30 @@ HIER_OBS_LEAVES = OrderedDict([("prop", (99,)), ("prop_a", (36,)), ("percep_2d",
                                ("target", (3,))])
 
 
+def _recurrent_records(rows, leaves, actions, cols, initial_state, first_mask, bootstrap_value, gamma, lam):
+    """Learner tensors of the learner's `rows` [T, N, width] of a recurrent unroll, in order: the observation `leaves` [T, N, *leaf], the
+    level's `actions` ((name, [T, N] tensor) pairs), `neglogp`, `discount`, `r`, `V`, `R` (lambda-returns), `M` (the mask each forward
+    received) and `S` = `initial_state`; `cols` = the record's (neglogp, reward, done, value) columns."""
+    T, N = rows.shape[:2]
+    out = OrderedDict()
+    c = 0
+    for name, shape in leaves.items():
+        k = int(np.prod(shape))
+        out[name] = rows[:, :, c:c + k].reshape(T, N, *shape)
+        c += k
+    out.update(actions)
+    neglogp, r, done, v = (rows[:, :, k] for k in cols)
+    discount = gamma * (1.0 - done)
+    out["neglogp"], out["discount"], out["r"], out["V"] = neglogp, discount, r, v
+    out["R"] = lambda_returns(r, discount, v, bootstrap_value.to(rows.dtype), lam)
+    mask = torch.empty((T, N), dtype=rows.dtype, device=rows.device)
+    mask[0] = (first_mask != 0).to(rows.dtype)
+    mask[1:] = (done[:-1] != 0).to(rows.dtype)
+    out["M"] = mask
+    out["S"] = initial_state
+    return out
+
+
 def hier_slab_records(slab, initial_state, first_mask, bootstrap_value, gamma=GAMMA, lam=LAM):
     """Learner tensors of an environmental-level unroll (`HierRolloutWorker.finish_unroll()`), on the slab's device, named:
     the observation leaves [T, N, *leaf], `A_Z` [T, N] int64 (the sampled code), `neglogp`, `discount` = gamma (1 - done), `r`,
@@ -86,39 +110,14 @@ def hier_slab_records(slab, initial_state, first_mask, bootstrap_value, gamma=GA
     M[t] = done[t-1]) -- all [T, N] float32 -- and `S` [N, 128], the recurrent state the unroll started from (code LSTM [c, h], then
     value LSTM [c, h])."""
     assert slab.dim() == 3 and slab.shape[2] == HIER_TRAJ_WIDTH, "expected a [T, N, %d] trajectory slab" % HIER_TRAJ_WIDTH
-    out = _recurrent_records(slab, HIER_OBS_LEAVES, slab[:, :, HCOL_DONE], slab[:, :, HCOL_REWARD], slab[:, :, HCOL_VALUE], first_mask,
-                             bootstrap_value, gamma, lam)
-    head = OrderedDict((k, out.pop(k)) for k in HIER_OBS_LEAVES)
-    head["A_Z"] = slab[:, :, HCOL_CODE].to(torch.int64)
-    head["neglogp"] = slab[:, :, HCOL_NEGLOGP]
-    head.update(out)
-    head["S"] = initial_state
-    return head
+    return _recurrent_records(slab, HIER_OBS_LEAVES, [("A_Z", slab[:, :, HCOL_CODE].to(torch.int64))],
+                              (HCOL_NEGLOGP, HCOL_REWARD, HCOL_DONE, HCOL_VALUE), initial_state, first_mask, bootstrap_value, gamma, lam)
 
 
 # observation leaves of the strategic level (CTG:111-124), in the order of its 965 observation columns
 SEPMC_OBS_LEAVES = OrderedDict([("prop", (99,)), ("prop_a", (36,)), ("percept_2d", (25, 13)), ("percept_1d", (128,)), ("percept_front", (25, 13)),
                                 ("percept_vec", (5,)), ("oppo_info", (15,)), ("oppo_info_cheat", (15,)), ("flag_info", (7,)),
                                 ("flag_info_cheat", (7,)), ("with_flag", (2,)), ("control_spd", (1,))])
-
-
-def _recurrent_records(slab, leaves, done, r, v, first_mask, bootstrap_value, gamma, lam):
-    """The observation leaves [T, N, *leaf] and discount, r, V, R (lambda-returns), M (the mask each forward received) of an unroll."""
-    T, N = done.shape
-    out = OrderedDict()
-    c = 0
-    for name, shape in leaves.items():
-        k = int(np.prod(shape))
-        out[name] = slab[:, :, c:c + k].reshape(T, N, *shape)
-        c += k
-    discount = gamma * (1.0 - done)
-    out["discount"], out["r"], out["V"] = discount, r, v
-    out["R"] = lambda_returns(r, discount, v, bootstrap_value.to(slab.dtype), lam)
-    mask = torch.empty((T, N), dtype=slab.dtype, device=slab.device)
-    mask[0] = (first_mask != 0).to(slab.dtype)
-    mask[1:] = (done[:-1] != 0).to(slab.dtype)
-    out["M"] = mask
-    return out
 
 
 def sepmc_slab_records(slab, initial_state, first_mask, bootstrap_value, gamma=GAMMA, lam=LAM, with_opponent=False):
@@ -132,17 +131,11 @@ def sepmc_slab_records(slab, initial_state, first_mask, bootstrap_value, gamma=G
     assert slab.dim() == 3 and slab.shape[2] == SEPMC_TRAJ_WIDTH and slab.shape[1] % 2 == 0, \
         "expected a [T, 2P, %d] trajectory slab" % SEPMC_TRAJ_WIDTH
     s0 = slab[:, 0::2]
-    out = _recurrent_records(s0, SEPMC_OBS_LEAVES, s0[:, :, SCOL_DONE], s0[:, :, SCOL_REWARD], s0[:, :, SCOL_VALUE], first_mask, bootstrap_value,
-                             gamma, lam)
-    head = OrderedDict((k, out.pop(k)) for k in SEPMC_OBS_LEAVES)
-    head["A_HLC"] = s0[:, :, SCOL_HEADING]
-    head["A_Z"] = s0[:, :, SCOL_CODE].to(torch.int64)
-    head["neglogp"] = s0[:, :, SCOL_NEGLOGP]
-    head.update(out)
-    head["S"] = initial_state
+    out = _recurrent_records(s0, SEPMC_OBS_LEAVES, [("A_HLC", s0[:, :, SCOL_HEADING]), ("A_Z", s0[:, :, SCOL_CODE].to(torch.int64))],
+                             (SCOL_NEGLOGP, SCOL_REWARD, SCOL_DONE, SCOL_VALUE), initial_state, first_mask, bootstrap_value, gamma, lam)
     if with_opponent:
-        head["opponent"] = s0[:, :, SCOL_OPPONENT].to(torch.int64)
-    return head
+        out["opponent"] = s0[:, :, SCOL_OPPONENT].to(torch.int64)
+    return out
 
 
 def slab_to_unrolls(slab, model_key, infos=None, **kw):

@@ -25,6 +25,8 @@ corridors on the engine (DESIGN.md 6).
 0-1 prop running mean / std | 2-46 value tower (unused here except by `value`) | 47-48 prop embed | 49-76 command encoder |
 77-78 embed | 79-87 LSTM | 88-89 logits | 90 codebook | 91-100 low-level controller | 101 logstd
 """
+import ctypes as C
+
 import numpy as np
 
 
@@ -360,7 +362,6 @@ def strategic_train_role_arrays():
 
 
 def _policy_lib():
-    import ctypes as C
     import os
     from .policy import POLICY_LIB_PATH
     if not os.path.exists(POLICY_LIB_PATH):
@@ -378,149 +379,132 @@ def _weight_blob(weights):
     return np.concatenate(w), starts
 
 
-class DeviceHierPolicy:
+def _blob_and_tables(models, *roles):
+    """(blob, tables): the arrays of all `models` in one fp32 blob, model after model (each laid out by `_weight_blob`), and for each list
+    of array indices in `roles` the int32 table of where those arrays start in the blob, model after model (the role tables of
+    include/llq_policy.h)."""
+    blobs, starts, base = [], [], 0
+    for m in models:
+        blob, s = _weight_blob(m)
+        blobs.append(blob)
+        starts.append(s + base)
+        base += blob.size
+    blob = np.concatenate(blobs) if blobs else np.zeros(0, np.float32)
+    return blob, [np.array([s[i] for s in starts for i in r], np.int32) for r in roles]
+
+
+def _vp(a):
+    return a.ctypes.data_as(C.c_void_p)
+
+
+class _HierHandle:
+    """One handle of csrc/llq_policy_hier.cu (include/llq_policy.h): the library, its calls and `close`."""
+
+    def __init__(self, create, *args):
+        """`create`(*args, &handle): the library entry that makes the handle."""
+        self.lib, self._h = _policy_lib(), None
+        h = C.c_void_p()
+        self._call(create, *args, C.byref(h))
+        self._h = h
+
+    def _call(self, entry, *args, error=RuntimeError):
+        """The library's `entry`(*args); a non-zero return raises `error` with the library's last error."""
+        if getattr(self.lib, entry)(*args):
+            raise error("%s: %s" % (entry, self.lib.llq_hier_policy_last_error().decode()))
+
+    def close(self):
+        if self._h:
+            self.lib.llq_hier_policy_destroy(self._h)
+            self._h = None
+
+
+class DeviceHierPolicy(_HierHandle):
     """The environmental- / strategic-level policy on the GPU (csrc/llq_policy_hier.cu through include/llq_policy.h): reads the engine's
     observation rows in place, keeps the LSTM states on the device, writes the actions the fused env step consumes.
     `train=True` (environmental level only): the training handle, stepped with `forward_rec` (sampled code, -log p, V; state rows of
     128 floats = code LSTM, then value LSTM); the strategic level's training handle is `DeviceSepmcTrainPolicy`."""
 
     def __init__(self, weights, device=0, train=False):
-        import ctypes as C
-        self._C, self.lib = C, _policy_lib()
-        self.strategic = len(weights) == 152
         assert len(weights) in (102, 152), "expected an environmental-level (102 arrays) or a strategic-level (152 arrays) model"
-        blob, starts = _weight_blob(weights)
-        off = np.array([starts[i] for i in hier_role_arrays(self.strategic)], np.int32)
-        h = C.c_void_p()
-        self.train = bool(train)
+        self.strategic, self.train = len(weights) == 152, bool(train)
         if self.train:
-            voff = np.array([starts[i] for i in hier_role_arrays(False, value_tower=True)], np.int32)      # a strategic handle is refused
-            rc = self.lib.llq_hier_policy_create_train(blob.ctypes.data_as(C.c_void_p), C.c_int64(blob.size), off.ctypes.data_as(C.c_void_p),
-                                                       C.c_int32(off.size), voff.ctypes.data_as(C.c_void_p), C.c_int32(voff.size),
-                                                       C.c_int32(int(self.strategic)), C.c_int32(device), C.byref(h))
+            blob, (off, voff) = _blob_and_tables([weights], hier_role_arrays(self.strategic), hier_role_arrays(False, value_tower=True))
+            super().__init__("llq_hier_policy_create_train", _vp(blob), C.c_int64(blob.size), _vp(off), C.c_int32(off.size), _vp(voff),
+                             C.c_int32(voff.size), C.c_int32(int(self.strategic)), C.c_int32(device))      # a strategic handle is refused
         else:
-            rc = self.lib.llq_hier_policy_create(blob.ctypes.data_as(C.c_void_p), C.c_int64(blob.size), off.ctypes.data_as(C.c_void_p),
-                                                 C.c_int32(off.size), C.c_int32(int(self.strategic)), C.c_int32(device), C.byref(h))
-        if rc:
-            raise RuntimeError("llq_hier_policy_create%s: %s" % ("_train" if self.train else "", self.lib.llq_hier_policy_last_error().decode()))
-        self._h = h
+            blob, (off,) = _blob_and_tables([weights], hier_role_arrays(self.strategic))
+            super().__init__("llq_hier_policy_create", _vp(blob), C.c_int64(blob.size), _vp(off), C.c_int32(off.size),
+                             C.c_int32(int(self.strategic)), C.c_int32(device))
         self.state_dim = 128 if (self.strategic or self.train) else 64
         self.obs_dim = 965 if self.strategic else 916
 
     def forward(self, obs_ptr, obs_ld, n, done_ptr, state_ptr, act_ptr, codes_ptr=None, heading_ptr=None, stream=None):
-        C = self._C
-        rc = self.lib.llq_hier_policy_forward(self._h, C.c_void_p(obs_ptr), C.c_int64(obs_ld), C.c_int32(n), C.c_void_p(done_ptr or 0), C.c_void_p(state_ptr),
-                                              C.c_void_p(act_ptr), C.c_void_p(codes_ptr or 0), C.c_void_p(heading_ptr or 0), C.c_void_p(stream or 0))
-        if rc:
-            raise RuntimeError("llq_hier_policy_forward: %s" % self.lib.llq_hier_policy_last_error().decode())
+        self._call("llq_hier_policy_forward", self._h, C.c_void_p(obs_ptr), C.c_int64(obs_ld), C.c_int32(n), C.c_void_p(done_ptr or 0),
+                   C.c_void_p(state_ptr), C.c_void_p(act_ptr), C.c_void_p(codes_ptr or 0), C.c_void_p(heading_ptr or 0), C.c_void_p(stream or 0))
 
     def forward_rec(self, obs_ptr, obs_ld, n, done_ptr, state_ptr, act_ptr, codes_ptr, values_ptr, neglogp_ptr, out_ld, seed, counter, row_gid0=0,
                     stream=None):
         """Training step (include/llq_policy.h, llq_hier_policy_forward_rec): sampled code -> codes_ptr (int32), V / -log p of row i ->
         values_ptr / neglogp_ptr + i * out_ld floats; the Gumbel noise is keyed by (row_gid0 + i, counter) and `seed`."""
-        C = self._C
-        rc = self.lib.llq_hier_policy_forward_rec(self._h, C.c_void_p(obs_ptr), C.c_int64(obs_ld), C.c_int32(n), C.c_void_p(done_ptr or 0),
-                                                  C.c_void_p(state_ptr), C.c_void_p(act_ptr), C.c_void_p(codes_ptr or 0), C.c_void_p(values_ptr or 0),
-                                                  C.c_void_p(neglogp_ptr or 0), C.c_int64(out_ld), C.c_uint64(seed), C.c_uint64(counter),
-                                                  C.c_int64(row_gid0), C.c_void_p(stream or 0))
-        if rc:
-            raise RuntimeError("llq_hier_policy_forward_rec: %s" % self.lib.llq_hier_policy_last_error().decode())
-
-    def close(self):
-        if self._h:
-            self.lib.llq_hier_policy_destroy(self._h)
-            self._h = None
+        self._call("llq_hier_policy_forward_rec", self._h, C.c_void_p(obs_ptr), C.c_int64(obs_ld), C.c_int32(n), C.c_void_p(done_ptr or 0),
+                   C.c_void_p(state_ptr), C.c_void_p(act_ptr), C.c_void_p(codes_ptr or 0), C.c_void_p(values_ptr or 0), C.c_void_p(neglogp_ptr or 0),
+                   C.c_int64(out_ld), C.c_uint64(seed), C.c_uint64(counter), C.c_int64(row_gid0), C.c_void_p(stream or 0))
 
 
-class DeviceSepmcTrainPolicy(DeviceHierPolicy):
+class DeviceSepmcTrainPolicy(_HierHandle):
     """The strategic level's training handle on the GPU (include/llq_policy.h, llq_hier_policy_create_train_strategic): `forward_rec`
     samples the heading, writes it raw with its -log p and V, and runs the frozen code controller (argmax code) and decoder on the
     clipped heading.  State rows of 192 floats: heading LSTM, code LSTM, value LSTM ([c, h] each)."""
 
     def __init__(self, weights, device=0):
-        import ctypes as C
-        self._C, self.lib = C, _policy_lib()
         assert len(weights) == 152, "expected a strategic-level model (152 arrays)"
         self.strategic, self.train = True, True
-        blob, starts = _weight_blob(weights)
-        off = np.array([starts[i] for i in hier_role_arrays(True)], np.int32)
-        toff = np.array([starts[i] for i in strategic_train_role_arrays()], np.int32)
-        h = C.c_void_p()
-        rc = self.lib.llq_hier_policy_create_train_strategic(blob.ctypes.data_as(C.c_void_p), C.c_int64(blob.size), off.ctypes.data_as(C.c_void_p),
-                                                             C.c_int32(off.size), toff.ctypes.data_as(C.c_void_p), C.c_int32(toff.size),
-                                                             C.c_int32(device), C.byref(h))
-        if rc:
-            raise RuntimeError("llq_hier_policy_create_train_strategic: %s" % self.lib.llq_hier_policy_last_error().decode())
-        self._h = h
+        blob, (off, toff) = _blob_and_tables([weights], hier_role_arrays(True), strategic_train_role_arrays())
+        super().__init__("llq_hier_policy_create_train_strategic", _vp(blob), C.c_int64(blob.size), _vp(off), C.c_int32(off.size), _vp(toff),
+                         C.c_int32(toff.size), C.c_int32(device))
         self.state_dim, self.obs_dim = 192, 965
+
+    # the deterministic entry, which the library refuses for this handle: `forward` raises the library's RuntimeError (naming
+    # llq_hier_policy_forward_rec_strategic, the entry to step with) rather than an AttributeError
+    forward = DeviceHierPolicy.forward
 
     def forward_rec(self, obs_ptr, obs_ld, n, done_ptr, state_ptr, act_ptr, codes_ptr, heading_ptr, values_ptr, neglogp_ptr, out_ld, seed, counter,
                     row_gid0=0, stream=None):
         """Training step (include/llq_policy.h, llq_hier_policy_forward_rec_strategic): raw sampled heading / V / -log p of row i ->
         heading_ptr / values_ptr / neglogp_ptr + i * out_ld floats, argmax code -> codes_ptr (int32); the heading noise is keyed by
         (row_gid0 + i, counter) and `seed`."""
-        C = self._C
-        rc = self.lib.llq_hier_policy_forward_rec_strategic(self._h, C.c_void_p(obs_ptr), C.c_int64(obs_ld), C.c_int32(n), C.c_void_p(done_ptr or 0),
-                                                            C.c_void_p(state_ptr), C.c_void_p(act_ptr), C.c_void_p(codes_ptr or 0),
-                                                            C.c_void_p(heading_ptr or 0), C.c_void_p(values_ptr or 0), C.c_void_p(neglogp_ptr or 0),
-                                                            C.c_int64(out_ld), C.c_uint64(seed), C.c_uint64(counter), C.c_int64(row_gid0),
-                                                            C.c_void_p(stream or 0))
-        if rc:
-            raise RuntimeError("llq_hier_policy_forward_rec_strategic: %s" % self.lib.llq_hier_policy_last_error().decode())
+        self._call("llq_hier_policy_forward_rec_strategic", self._h, C.c_void_p(obs_ptr), C.c_int64(obs_ld), C.c_int32(n), C.c_void_p(done_ptr or 0),
+                   C.c_void_p(state_ptr), C.c_void_p(act_ptr), C.c_void_p(codes_ptr or 0), C.c_void_p(heading_ptr or 0), C.c_void_p(values_ptr or 0),
+                   C.c_void_p(neglogp_ptr or 0), C.c_int64(out_ld), C.c_uint64(seed), C.c_uint64(counter), C.c_int64(row_gid0), C.c_void_p(stream or 0))
 
 
-class DeviceOpponentPool:
+class DeviceOpponentPool(_HierHandle):
     """K frozen strategic-level models on the GPU in one handle (include/llq_policy.h, llq_hier_policy_create_pool): `forward` draws a
     new model for every row whose done flag is set, from the probabilities of `set_probs` (uniform until then), and runs every row's
     deterministic forward with its own model in one launch.  `models`: a list of 1 .. 64 strategic-level models (152 arrays each);
     `max_rows` bounds the rows of every forward.  Single-owner: the handle holds one workspace, so one stream at a time."""
 
     def __init__(self, models, device=0, *, max_rows, probs=None):
-        import ctypes as C
-        self._C, self.lib = C, _policy_lib()
-        self._h = None
         assert all(len(m) == 152 for m in models), "expected strategic-level models (152 arrays)"
-        blobs, offs, base = [], [], 0
-        for m in models:
-            blob, starts = _weight_blob(m)
-            offs.append(np.array([starts[i] for i in hier_role_arrays(True)], np.int64) + base)
-            blobs.append(blob)
-            base += blob.size
-        blob = np.concatenate(blobs) if blobs else np.zeros(0, np.float32)
-        off = np.concatenate(offs).astype(np.int32) if offs else np.zeros(0, np.int32)
-        h = C.c_void_p()
-        rc = self.lib.llq_hier_policy_create_pool(blob.ctypes.data_as(C.c_void_p), C.c_int64(blob.size), off.ctypes.data_as(C.c_void_p),
-                                                  C.c_int32(len(models)), C.c_int32(int(max_rows)), C.c_int32(device), C.byref(h))
-        if rc:
-            raise RuntimeError("llq_hier_policy_create_pool: %s" % self.lib.llq_hier_policy_last_error().decode())
-        self._h = h
         self.strategic, self.train = True, False
         self.n_models, self.max_rows = len(models), int(max_rows)
         self.state_dim, self.obs_dim = 128, 965
+        blob, (off,) = _blob_and_tables(models, hier_role_arrays(True))
+        super().__init__("llq_hier_policy_create_pool", _vp(blob), C.c_int64(blob.size), _vp(off), C.c_int32(self.n_models), C.c_int32(self.max_rows),
+                         C.c_int32(device))
         if probs is not None:
             self.set_probs(probs)
 
     def set_probs(self, probs):
         """Draw probabilities of the next forwards: one finite entry >= 0 per model, positive sum (they need not sum to 1)."""
-        C = self._C
         p = np.ascontiguousarray(probs, np.float64).reshape(-1)
-        rc = self.lib.llq_hier_policy_set_pool_probs(self._h, p.ctypes.data_as(C.c_void_p), C.c_int32(p.size))
-        if rc:
-            raise ValueError("llq_hier_policy_set_pool_probs: %s" % self.lib.llq_hier_policy_last_error().decode())
+        self._call("llq_hier_policy_set_pool_probs", self._h, _vp(p), C.c_int32(p.size), error=ValueError)
 
     def forward(self, obs_ptr, obs_ld, n, done_ptr, state_ptr, act_ptr, codes_ptr, heading_ptr, model_ptr, model_rec_ptr, rec_ld, seed, counter,
                 row_gid0=0, stream=None):
         """One step (include/llq_policy.h, llq_hier_policy_forward_pool): rows with done set draw a model into model_ptr (int32[n]), keyed
         by (row_gid0 + i, counter) and `seed`; model_rec_ptr + i * rec_ld floats (nullable) records every row's model."""
-        C = self._C
-        rc = self.lib.llq_hier_policy_forward_pool(self._h, C.c_void_p(obs_ptr), C.c_int64(obs_ld), C.c_int32(n), C.c_void_p(done_ptr or 0),
-                                                   C.c_void_p(state_ptr), C.c_void_p(act_ptr), C.c_void_p(codes_ptr or 0), C.c_void_p(heading_ptr or 0),
-                                                   C.c_void_p(model_ptr), C.c_void_p(model_rec_ptr or 0), C.c_int64(rec_ld), C.c_uint64(seed),
-                                                   C.c_uint64(counter), C.c_int64(row_gid0), C.c_void_p(stream or 0))
-        if rc:
-            raise RuntimeError("llq_hier_policy_forward_pool: %s" % self.lib.llq_hier_policy_last_error().decode())
-
-    def close(self):
-        if self._h:
-            self.lib.llq_hier_policy_destroy(self._h)
-            self._h = None
+        self._call("llq_hier_policy_forward_pool", self._h, C.c_void_p(obs_ptr), C.c_int64(obs_ld), C.c_int32(n), C.c_void_p(done_ptr or 0),
+                   C.c_void_p(state_ptr), C.c_void_p(act_ptr), C.c_void_p(codes_ptr or 0), C.c_void_p(heading_ptr or 0), C.c_void_p(model_ptr),
+                   C.c_void_p(model_rec_ptr or 0), C.c_int64(rec_ld), C.c_uint64(seed), C.c_uint64(counter), C.c_int64(row_gid0),
+                   C.c_void_p(stream or 0))

@@ -1,5 +1,5 @@
 """Row f3: TLeague-format unrolls from a trajectory slab (parallel/unroll.py; distill_actor.py:164-167, pmc_net_data.py:7-16)
-and the on-device actor loop that fills the slab (parallel/rollout.py)."""
+and the on-device actor loops that fill the slab (parallel/rollout.py)."""
 import numpy as np
 import pytest
 import torch
@@ -116,3 +116,24 @@ def test_rollout_worker_records_are_aligned(built):
     unrolls = slab_to_unrolls(torch.from_numpy(slab), "m", gamma=0.95, lam=0.95)
     assert len(unrolls) == n and unrolls[0][1].size == 2 * T * RECORD_WIDTH
     pol.close(); eng.close(); chk.close()
+
+
+@pytest.mark.gpu
+def test_workers_refuse_an_engine_without_auto_reset(built):
+    """The workers step through the engine's auto-reset: an engine with auto_reset=0 is refused before anything is allocated."""
+    from lifelike_agility_and_play_b200 import _capi as capi
+    from lifelike_agility_and_play_b200.model.compile_model import load_model_blob
+    from lifelike_agility_and_play_b200.mocap import synthetic_mocap
+    from lifelike_agility_and_play_b200.parallel import HierRolloutWorker, RolloutWorker
+    from lifelike_agility_and_play_b200.policy import DevicePolicy
+    from lifelike_agility_and_play_b200.policy_epmc import DeviceHierPolicy, random_weights as hier_weights
+    from test_policy import random_weights
+    lib, blob = capi.load_cuda_library(), load_model_blob()
+    pmc = capi.VecEngine(lib, 8, blob, synthetic_mocap(2, seed=2, min_frames=380, max_frames=420), seed=21, device=0, auto_reset=0)
+    epmc = capi.VecEngine(lib, 8, blob, None, device=0, env_kind=capi.ENV_EPMC, auto_reset=0)
+    pol, hpol = DevicePolicy(random_weights(9), device=0), DeviceHierPolicy(hier_weights(False, 0), device=0, train=True)
+    with pytest.raises(ValueError, match="auto_reset=1"):
+        RolloutWorker(pmc, pol, 4, "cuda:0")
+    with pytest.raises(ValueError, match="auto_reset=1"):
+        HierRolloutWorker(epmc, hpol, 4, "cuda:0")
+    pol.close(); hpol.close(); pmc.close(); epmc.close()

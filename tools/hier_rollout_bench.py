@@ -1,8 +1,8 @@
 """Timing of the environmental level's training rollouts on the GPU: the hierarchical policy kernel's deterministic forward
 (llq_hier_policy_forward) and training forward (llq_hier_policy_forward_rec: value tower, Gumbel sample, -log p), and the env-steps/s of
 `HierRolloutWorker` (training forward + fused step + reset per step), at 8192 EPMC envs on elements 0 and 3 with random weights of the
-shipped architecture.  Steady state: one unroll of pre-roll before any timed window; CUDA events on the stream the work runs on.  The
-card's name and power limit are read in the same run.  Prints one JSON line.
+shipped architecture.  Steady state: one unroll of pre-roll before any timed window (`worker_rate`, which the strategic level's tools
+share); CUDA events on the stream the work runs on.  The card's name and power limit are read in the same run.  Prints one JSON line.
 
     python tools/hier_rollout_bench.py [--envs 8192] [--unroll 32] [--unrolls 4] [--reps 50]
 """
@@ -53,6 +53,26 @@ def timed(fn, stream, reps):
     return e0.elapsed_time(e1) / reps
 
 
+def worker_rate(worker, first_obs, unrolls):
+    """Milliseconds per step of a rollout worker: one unroll of pre-roll (module loads, a full unroll of episodes under way), then
+    `unrolls` unrolls between CUDA events on the worker's stream.  Returns (ms per step, the pre-roll's slab view, which the timed
+    unrolls have refilled since with later records); everything has finished on return."""
+    import torch
+    worker.start(first_obs)
+    for _ in range(worker.T):
+        worker.step()
+    slab = worker.finish_unroll().slab
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(worker.stream)
+    for _ in range(unrolls):
+        for _ in range(worker.T):
+            worker.step()
+        worker.finish_unroll()
+    e1.record(worker.stream)
+    e1.synchronize()
+    return e0.elapsed_time(e1) / (worker.T * unrolls), slab
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--envs", type=int, default=8192)
@@ -73,12 +93,9 @@ def main():
     for element in (0, 3):
         eng = epmc_engine(n, element)
         worker = HierRolloutWorker(eng, tr, a.unroll, "cuda:0", seed=3)
-        worker.start(eng.reset())
-        for _ in range(a.unroll):                               # pre-roll: module loads, a full unroll of episodes under way
-            worker.step()
-        slab = worker.finish_unroll().slab
+        ms, slab = worker_rate(worker, eng.reset(), a.unrolls)
         st = worker.stream
-        # the two forwards on the pre-rolled observations, on the worker's stream
+        # the two forwards on rolled-out observations, on the worker's stream
         obs = slab[a.unroll - 1]
         s64, s128 = torch.zeros((n, 64), device="cuda"), torch.zeros((n, 128), device="cuda")
         act, codes = torch.zeros((n, 12), device="cuda"), torch.zeros((n,), dtype=torch.int32, device="cuda")
@@ -88,19 +105,9 @@ def main():
                                                 st.cuda_stream), st, a.reps)
             t_tr = timed(lambda i: tr.forward_rec(obs.data_ptr(), obs.shape[1], n, None, s128.data_ptr(), act.data_ptr(), codes.data_ptr(),
                                                   val.data_ptr(), nlp.data_ptr(), 1, 3, 10 ** 6 + i, 0, st.cuda_stream), st, a.reps)
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record(st)
-        for _ in range(a.unrolls):
-            for _ in range(a.unroll):
-                worker.step()
-            worker.finish_unroll()
-        e1.record(st)
-        e1.synchronize()
-        ms = e0.elapsed_time(e1)
         out["element%d" % element] = {"forward_deterministic_ms": round(t_det, 4), "forward_training_ms": round(t_tr, 4),
                                       "training_over_deterministic": round(t_tr / t_det, 3),
-                                      "worker_env_steps_per_s": round(n * a.unroll * a.unrolls / (ms / 1e3)),
-                                      "worker_ms_per_step": round(ms / (a.unroll * a.unrolls), 4)}
+                                      "worker_env_steps_per_s": round(n / (ms / 1e3)), "worker_ms_per_step": round(ms, 4)}
         eng.close()
     det.close(); tr.close()
     print(json.dumps(out))

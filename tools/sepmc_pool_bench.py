@@ -17,34 +17,20 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-from hier_rollout_bench import card, timed  # noqa: E402
+from hier_rollout_bench import card, timed, worker_rate  # noqa: E402
 from sepmc_rollout_bench import sepmc_engine  # noqa: E402
 
 
-def worker_rate(opponent, pairs, unroll, unrolls):
+def opponent_rate(opponent, pairs, unroll, unrolls):
+    """Pair-steps/s of SepmcRolloutWorker against `opponent`, and the [2P, 984] records of one step of the run."""
     from lifelike_agility_and_play_b200.parallel import SepmcRolloutWorker
     from lifelike_agility_and_play_b200.policy_epmc import DeviceSepmcTrainPolicy, random_weights
-    import torch
     tr = DeviceSepmcTrainPolicy(random_weights(True, 1), device=0)
     eng = sepmc_engine(2 * pairs)
-    worker = SepmcRolloutWorker(eng, tr, opponent, unroll, "cuda:0", seed=3)
-    worker.start(eng.reset())
-    for _ in range(unroll):                                     # pre-roll: module loads, a full unroll of games under way
-        worker.step()
-    slab = worker.finish_unroll().slab
-    st = worker.stream
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record(st)
-    for _ in range(unrolls):
-        for _ in range(unroll):
-            worker.step()
-        worker.finish_unroll()
-    e1.record(st)
-    e1.synchronize()
-    ms = e0.elapsed_time(e1)
+    ms, slab = worker_rate(SepmcRolloutWorker(eng, tr, opponent, unroll, "cuda:0", seed=3), eng.reset(), unrolls)
     obs = slab[unroll - 1].clone()
     eng.close(); tr.close()
-    return round(pairs * unroll * unrolls / (ms / 1e3)), obs
+    return round(pairs / (ms / 1e3)), obs
 
 
 def main():
@@ -63,9 +49,9 @@ def main():
     out = {"gpu": name, "power_limit": power, "rows": a.rows, "pairs": a.pairs, "unroll": a.unroll}
     models = [random_weights(True, 10 + k) for k in range(64)]
     one = DeviceHierPolicy(models[0], device=0)
-    rate1, last = worker_rate(one, a.pairs, a.unroll, a.unrolls)
+    rate1, last = opponent_rate(one, a.pairs, a.unroll, a.unrolls)
     pool16 = DeviceOpponentPool(models[:16], device=0, max_rows=a.pairs)
-    rate16, _ = worker_rate(pool16, a.pairs, a.unroll, a.unrolls)
+    rate16, _ = opponent_rate(pool16, a.pairs, a.unroll, a.unrolls)
     pool16.close()
     out.update({"worker_pair_steps_per_s_one_opponent": rate1, "worker_pair_steps_per_s_pool16": rate16})
     n = a.rows

@@ -16,7 +16,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-from hier_rollout_bench import card, timed  # noqa: E402
+from hier_rollout_bench import card, timed, worker_rate  # noqa: E402
 
 
 def sepmc_engine(n_robots):
@@ -48,12 +48,9 @@ def main():
     out = {"gpu": name, "power_limit": power, "rows": a.rows, "pairs": a.pairs, "unroll": a.unroll}
     eng = sepmc_engine(2 * a.pairs)
     worker = SepmcRolloutWorker(eng, tr, opp, a.unroll, "cuda:0", seed=3)
-    worker.start(eng.reset())
-    for _ in range(a.unroll):                                   # pre-roll: module loads, a full unroll of games under way
-        worker.step()
-    slab = worker.finish_unroll().slab
+    ms, slab = worker_rate(worker, eng.reset(), a.unrolls)
     st = worker.stream
-    # the two forwards on pre-rolled observations (rows of the last record, repeated up to --rows), on the worker's stream
+    # the two forwards on rolled-out observations (rows of the last record, repeated up to --rows), on the worker's stream
     n = a.rows
     obs = slab[a.unroll - 1].repeat((n + slab.shape[1] - 1) // slab.shape[1], 1)[:n].contiguous()
     s128, s192 = torch.zeros((n, 128), device="cuda"), torch.zeros((n, 192), device="cuda")
@@ -64,19 +61,9 @@ def main():
                                             st.cuda_stream), st, a.reps)
         t_tr = timed(lambda i: tr.forward_rec(obs.data_ptr(), obs.shape[1], n, None, s192.data_ptr(), act.data_ptr(), codes.data_ptr(), hd.data_ptr(),
                                               val.data_ptr(), nlp.data_ptr(), 1, 3, 10 ** 6 + i, 0, st.cuda_stream), st, a.reps)
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record(st)
-    for _ in range(a.unrolls):
-        for _ in range(a.unroll):
-            worker.step()
-        worker.finish_unroll()
-    e1.record(st)
-    e1.synchronize()
-    ms = e0.elapsed_time(e1)
     out.update({"forward_deterministic_ms": round(t_det, 4), "forward_training_ms": round(t_tr, 4),
                 "training_over_deterministic": round(t_tr / t_det, 3),
-                "worker_pair_steps_per_s": round(a.pairs * a.unroll * a.unrolls / (ms / 1e3)),
-                "worker_ms_per_step": round(ms / (a.unroll * a.unrolls), 4)})
+                "worker_pair_steps_per_s": round(a.pairs / (ms / 1e3)), "worker_ms_per_step": round(ms, 4)})
     eng.close(); det.close(); tr.close(); opp.close()
     print(json.dumps(out))
 
