@@ -27,7 +27,7 @@ extern "C" {
 
 typedef struct llq_policy* llq_policy_handle;
 
-/* Uploads the weights to `device`.  Returns 0 or a negative LLQ_E* code (llq.h); message via llq_policy_last_error(). */
+/* Uploads the weights to `device` and packs them there; returns once the handle is ready.  Returns 0 or a negative LLQ_E* code (llq.h); message via llq_policy_last_error(). */
 int llq_policy_create(const float* weights, int64_t n_weights, int32_t device, llq_policy_handle* out);
 int llq_policy_destroy(llq_policy_handle h);
 /* actions[n,12] = mean action for obs[n, >=207] (device pointers; obs_ld = row stride in floats); `codes` (int32[n], device,
@@ -47,6 +47,19 @@ int llq_policy_forward_ex(llq_policy_handle h, const float* d_obs, int64_t obs_l
  * shards with equal seeds draw different noise (one actor process per shard in the reference draws from its own np.random). */
 int llq_policy_forward_rec(llq_policy_handle h, const float* d_obs, int64_t obs_ld, int32_t n, float* d_actions, int32_t* d_codes,
                            float* d_values, float* d_neglogp, int64_t out_ld, uint64_t seed, uint64_t counter, int64_t row_gid0, void* stream);
+/* Model refresh (a training actor following its learner): the handle takes a new 28-array blob of the same layout as at create.
+ *   Ordering: asynchronous on `stream` (0 = the default stream); forwards queued on `stream` before the call see the old weights, forwards
+ *     queued after it the new ones.  Nothing synchronises the device; forwards on OTHER streams are not ordered with the refresh.
+ *   on_device = 0: `weights` is host memory, reusable as soon as the call returns: it is copied into a pinned staging buffer of the handle
+ *     and uploaded with cudaMemcpyAsync on `stream` into the handle's raw blob (1.4 MB of device memory kept since create).  A second
+ *     host refresh waits on the host (an event) until the previous upload has left the staging buffer: the only host wait, and only when
+ *     two refreshes are closer together than one copy.
+ *   on_device = 1: `weights` is device memory on the handle's device (e.g. a blob broadcast by the learner rank); host memory or another
+ *     device returns LLQ_EINVAL.  The caller keeps it alive until the refresh has run on `stream`.
+ *   The forward reads an image of the blob in MMA B-fragment order; the refresh rebuilds it in place with the same pack kernel as
+ *   llq_policy_create (a pure permutation with zero padding).  Null arguments, a wrong length or a bad on_device return LLQ_EINVAL
+ *   before the device is touched. */
+int llq_policy_set_weights(llq_policy_handle h, const float* weights, int64_t n_weights, int32_t on_device, void* stream);
 const char* llq_policy_last_error(void);
 
 /* ---- environmental- and strategic-level policies (csrc/llq_policy_hier.cu): conv encoders + layer-norm LSTMs + the frozen
@@ -147,6 +160,22 @@ int llq_hier_policy_set_pool_probs(llq_hier_policy_handle h, const double* probs
 int llq_hier_policy_forward_pool(llq_hier_policy_handle h, const float* d_obs, int64_t obs_ld, int32_t n, const uint8_t* d_done, float* d_state,
                                  float* d_actions, int32_t* d_codes, float* d_heading, int32_t* d_model, float* d_model_rec, int64_t rec_ld,
                                  uint64_t seed, uint64_t counter, int64_t row_gid0, void* stream);
+/* Model refresh of a hierarchical handle (deterministic, environmental training or strategic training; a pool handle is refused and
+ * pointed to llq_hier_policy_set_pool_model): the handle keeps the blob as given at create and its role tables hold offsets into it, so
+ * the refresh is one copy of a blob of the same architecture and file layout (n_weights must equal the length given at create; the
+ * role tables stay).  Ordering, on_device and the staging wait are those of llq_policy_set_weights.  The LSTM states are the caller's
+ * and are not touched: a row continues its episode with the new weights. */
+int llq_hier_policy_set_weights(llq_hier_policy_handle h, const float* weights, int64_t n_weights, int32_t on_device, void* stream);
+/* Replaces model k (0 <= k < n_models; K is fixed at create) of a pool handle.  Model k's region of the pool blob runs from its
+ * smallest role offset to the next larger model start (the smallest role offset of another model), or to the end of the blob; it is
+ * computed at create.  n_weights must equal the region's length and the new model must be laid out like the one it replaces
+ * (policy_epmc.DeviceOpponentPool lays every model out alike).  LLQ_EINVAL: k out of range, not a pool handle, or a pool whose models
+ * share arrays (two models starting at the same float, or an array of model k starting outside its region).  Ordering and sources as
+ * llq_hier_policy_set_weights.  Rows whose current game is against model k continue that game with the new weights and the state they
+ * already carry; draws are not touched.  To grow a league, create the pool with the capacity needed, give the unused models probability
+ * 0 (llq_hier_policy_set_pool_probs) and fill them later. */
+int llq_hier_policy_set_pool_model(llq_hier_policy_handle h, int32_t k, const float* weights, int64_t n_weights, int32_t on_device,
+                                   void* stream);
 const char* llq_hier_policy_last_error(void);
 
 #ifdef __cplusplus

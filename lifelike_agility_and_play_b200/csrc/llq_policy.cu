@@ -5,8 +5,8 @@
 // on the tensor cores as 3xTF32 (`mma.sync.m16n8k8.tf32`, fp32 accumulate): every operand is split into a TF32 head and a
 // remainder (truncation split) and the three significant products a_lo*b_hi + a_hi*b_lo + a_hi*b_hi are accumulated, which restores fp32-level
 // accuracy (the 12 outputs are joint targets for the physics and the parity bar is 1e-4, so plain TF32 -- a 1e-3 perturbation that
-// can also flip the discrete code -- is not an option).  The weights are re-ordered once, at llq_policy_create, into MMA
-// B-fragment order, so a warp fetches the fragments of a k-step with one coalesced 8-byte load per lane and n-tile; they stream
+// can also flip the discrete code -- is not an option).  The weights are re-ordered on the device (pmc_pack_kernel, at
+// llq_policy_create and at every llq_policy_set_weights) into MMA B-fragment order, so a warp fetches the fragments of a k-step with one coalesced 8-byte load per lane and n-tile; they stream
 // through L2 (1.4 MB per CTA) double-buffered in registers four k-steps ahead (LLQ_POLICY_KU).  An earlier version of this kernel
 // did the same layers with fp32 FFMA (one output neuron per thread, 32 accumulators).
 // The tile is 32 rows, not 128, on purpose: 4096 envs -> 128 CTAs = one wave over the H100's 132 SMs; a 128-row tile (one
@@ -285,14 +285,87 @@ __global__ void __launch_bounds__(THREADS) pmc_policy_kernel(const float* __rest
   }
 }
 
+// ---- the weight image: the 28 arrays of the blob re-ordered for pmc_policy_kernel.  Plain arrays are copied, every fully connected
+// layer becomes its B fragments ([ktile][ntile][lane] float2 = {W[8kt+t][8nt+g], W[8kt+t+4][8nt+g]}, zero outside [K) x [N)) and its
+// bias padded to the n-tiles, every piece starts on a 16-byte boundary and the gaps are zero.  The host computes only where the pieces
+// go (image_layout); pmc_pack_kernel writes the image from the raw blob in device memory, at create and at every refresh.
+enum PieceKind { P_PLAIN = 0, P_FRAG = 1, P_BIAS = 2 };
+struct Piece { int kind, src, dst, K, N; };   // P_PLAIN: K floats; P_FRAG: W[K][N]; P_BIAS: b[N]; all offsets in floats
+constexpr int kPieces = 28;                    // one per array of the blob
+struct Layout { Piece p[kPieces]; int total; };
+
+// piece blockIdx.y covers the image floats [dst, next piece's dst) (the last one up to total); every float of the image is written
+__global__ void __launch_bounds__(THREADS) pmc_pack_kernel(const float* __restrict__ raw, float* __restrict__ img, Layout L) {
+  const int pi = blockIdx.y;
+  const Piece P = L.p[pi];
+  const int end = pi + 1 < kPieces ? L.p[pi + 1].dst : L.total;
+  const int NT = (P.N + 7) >> 3;
+  for (int j = blockIdx.x * THREADS + threadIdx.x; P.dst + j < end; j += gridDim.x * THREADS) {
+    float v = 0.f;
+    if (P.kind == P_PLAIN) {
+      if (j < P.K) v = raw[P.src + j];
+    } else if (P.kind == P_BIAS) {
+      if (j < P.N) v = raw[P.src + j];
+    } else {
+      const int tile = j >> 6, lane = (j >> 1) & 31, kt = tile / NT, nt = tile - kt * NT;
+      const int k = kt * 8 + (lane & 3) + 4 * (j & 1), nn = nt * 8 + (lane >> 2);
+      if (k < P.K && nn < P.N) v = raw[P.src + k * P.N + nn];
+    }
+    img[P.dst + j] = v;
+  }
+}
+
+// where the pieces of the 28 arrays (include/llq_policy.h) go in the image: piece i holds array i; a zero total flags a mismatch
+Layout image_layout() {
+  Layout L{};
+  int src = 0, dst = 0, i = 0;
+  auto align = [&]() { dst = (dst + 3) & ~3; };
+  auto plain = [&](int cnt) { align(); L.p[i++] = Piece{P_PLAIN, src, dst, cnt, 0}; src += cnt; dst += cnt; };
+  auto layer = [&](int K, int N) {
+    const int KT = (K + 7) / 8, NT = (N + 7) / 8;
+    align(); L.p[i++] = Piece{P_FRAG, src, dst, K, N}; src += K * N; dst += KT * NT * 64;
+    align(); L.p[i++] = Piece{P_BIAS, src, dst, 0, N}; src += N; dst += NT * 8;
+  };
+  plain(N_PROP); plain(N_PROP); plain(N_FUT); plain(N_FUT);
+  layer(N_OBS, H); layer(H, H); plain(H); plain(1);
+  layer(N_OBS, H); layer(H, H); layer(H, Z); plain(Z * NCODE);
+  layer(N_PROP, PE); layer(Z, ZE); layer(PE + ZE, H); layer(H, H); layer(H, NACT);
+  plain(NACT);
+  L.total = dst;
+  return (i == kPieces && src == LLQ_POLICY_N_WEIGHTS) ? L : Layout{};
+}
+
 thread_local std::string g_err;
 int fail(int code, const char* msg) { g_err = msg; return code; }
 
 constexpr int SMEM_BYTES = (int)(sizeof(float) * (M * LDX + 2 * M * LDH));
+constexpr int kPackBlocks = 32;                // CTAs per piece: 8192 threads over at most 65 536 floats
 
 }  // namespace
 
-struct llq_policy { int device; float* d_w; Weights w; };
+// d_raw: the raw blob of the last create / host refresh (the pack kernel's source); h_stage: pinned host staging of host refreshes, its
+// copy to d_raw followed by ev_stage
+struct llq_policy {
+  int device; float* d_w; float* d_raw; Layout layout; Weights w;
+  float* h_stage = nullptr; cudaEvent_t ev_stage = nullptr; bool staged = false;
+};
+
+namespace {
+
+int pack(llq_policy* h, const float* d_src, cudaStream_t stream) {
+  pmc_pack_kernel<<<dim3(kPackBlocks, kPieces), THREADS, 0, stream>>>(d_src, h->d_w, h->layout);
+  const cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? LLQ_OK : fail(LLQ_ECUDA, cudaGetErrorString(e));
+}
+
+void release(llq_policy* h) {
+  cudaFree(h->d_w); cudaFree(h->d_raw);
+  if (h->h_stage) cudaFreeHost(h->h_stage);
+  if (h->ev_stage) cudaEventDestroy(h->ev_stage);
+  delete h;
+}
+
+}  // namespace
 
 extern "C" {
 
@@ -301,72 +374,72 @@ const char* llq_policy_last_error(void) { return g_err.c_str(); }
 int llq_policy_create(const float* weights, int64_t n_weights, int32_t device, llq_policy_handle* out) {
   if (!weights || !out) return fail(LLQ_EINVAL, "null argument");
   if (n_weights != LLQ_POLICY_N_WEIGHTS) return fail(LLQ_EINVAL, "weight blob has the wrong length (include/llq_policy.h)");
+  const Layout layout = image_layout();
+  if (layout.total == 0) return fail(LLQ_EINVAL, "internal: weight layout mismatch");
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(LLQ_ECUDA, "no CUDA device visible (no CPU fallback)");
   if (device < 0 || device >= ndev) return fail(LLQ_EINVAL, "device ordinal out of range");
   llq_policy* h = new (std::nothrow) llq_policy();
   if (!h) return fail(LLQ_ENOMEM, "out of memory");
-  h->device = device;
+  h->device = device; h->d_w = nullptr; h->d_raw = nullptr; h->layout = layout;
   cudaSetDevice(device);
-  // one host image: plain arrays copied, fully connected layers re-ordered into MMA B-fragment order, every piece 16-byte aligned
-  std::vector<float> img;
-  auto align = [&]() { while (img.size() & 3) img.push_back(0.f); };
-  const float* src = weights;
-  auto plain = [&](size_t cnt) { align(); const size_t o = img.size(); img.insert(img.end(), src, src + cnt); src += cnt; return o; };
-  struct LOff { size_t w, b; };
-  auto layer = [&](int K, int N) {      // consumes W[K][N] and b[N]
-    const int KT = (K + 7) / 8, NT = (N + 7) / 8;
-    align();
-    LOff o; o.w = img.size();
-    img.resize(img.size() + (size_t)KT * NT * 64, 0.f);
-    for (int kt = 0; kt < KT; kt++)
-      for (int nt = 0; nt < NT; nt++)
-        for (int lane = 0; lane < 32; lane++) {
-          const int g = lane >> 2, t = lane & 3, k0 = kt * 8 + t, k1 = k0 + 4, nn = nt * 8 + g;
-          float* d = &img[o.w + (((size_t)kt * NT + nt) * 32 + lane) * 2];
-          d[0] = (k0 < K && nn < N) ? src[(size_t)k0 * N + nn] : 0.f;
-          d[1] = (k1 < K && nn < N) ? src[(size_t)k1 * N + nn] : 0.f;
-        }
-    src += (size_t)K * N;
-    align();
-    o.b = img.size();
-    img.resize(img.size() + (size_t)NT * 8, 0.f);
-    for (int j = 0; j < N; j++) img[o.b + j] = src[j];
-    src += N;
-    return o;
-  };
-  const size_t o_pm = plain(N_PROP), o_ps = plain(N_PROP), o_fm = plain(N_FUT), o_fs = plain(N_FUT);
-  const LOff v1 = layer(N_OBS, H), v2 = layer(H, H);
-  const size_t o_v3w = plain(H), o_v3b = plain(1);
-  const LOff e1 = layer(N_OBS, H), e2 = layer(H, H), e3 = layer(H, Z);
-  const size_t o_code = plain((size_t)Z * NCODE);
-  const LOff pe = layer(N_PROP, PE), ze = layer(Z, ZE), d1 = layer(PE + ZE, H), d2 = layer(H, H), d3 = layer(H, NACT);
-  const size_t o_ls = plain(NACT);
-  if ((int64_t)(src - weights) != n_weights) { delete h; return fail(LLQ_EINVAL, "internal: weight layout mismatch"); }
-  if (cudaMalloc(&h->d_w, sizeof(float) * img.size()) != cudaSuccess) { delete h; return fail(LLQ_ECUDA, "cudaMalloc failed"); }
-  if (cudaMemcpy(h->d_w, img.data(), sizeof(float) * img.size(), cudaMemcpyHostToDevice) != cudaSuccess) {
-    cudaFree(h->d_w); delete h; return fail(LLQ_ECUDA, "weight upload failed");
+  // the raw blob goes up as it is, the pack kernel writes the image from it; the create returns once the image is complete
+  if (cudaMalloc(&h->d_w, sizeof(float) * layout.total) != cudaSuccess || cudaMalloc(&h->d_raw, sizeof(float) * LLQ_POLICY_N_WEIGHTS) != cudaSuccess) {
+    release(h); return fail(LLQ_ECUDA, "cudaMalloc failed");
   }
+  if (cudaMemcpy(h->d_raw, weights, sizeof(float) * LLQ_POLICY_N_WEIGHTS, cudaMemcpyHostToDevice) != cudaSuccess) {
+    release(h); return fail(LLQ_ECUDA, "weight upload failed");
+  }
+  if (pack(h, h->d_raw, 0) != LLQ_OK) { release(h); return LLQ_ECUDA; }
+  if (cudaStreamSynchronize(0) != cudaSuccess) { release(h); return fail(LLQ_ECUDA, "weight pack failed"); }
   const float* D = h->d_w;
-  auto L = [&](LOff o) { Layer l; l.w = reinterpret_cast<const float2*>(D + o.w); l.b = D + o.b; return l; };
+  const Piece* p = layout.p;
+  auto L = [&](int i) { Layer l; l.w = reinterpret_cast<const float2*>(D + p[i].dst); l.b = D + p[i + 1].dst; return l; };
   Weights& w = h->w;
-  w.prop_mean = D + o_pm; w.prop_std = D + o_ps; w.fut_mean = D + o_fm; w.fut_std = D + o_fs;
-  w.v1 = L(v1); w.v2 = L(v2); w.v3w = D + o_v3w; w.v3b = D + o_v3b;
-  w.e1 = L(e1); w.e2 = L(e2); w.e3 = L(e3); w.code = D + o_code;
-  w.pe = L(pe); w.ze = L(ze); w.d1 = L(d1); w.d2 = L(d2); w.d3 = L(d3);
-  w.logstd = D + o_ls;
+  w.prop_mean = D + p[0].dst; w.prop_std = D + p[1].dst; w.fut_mean = D + p[2].dst; w.fut_std = D + p[3].dst;
+  w.v1 = L(4); w.v2 = L(6); w.v3w = D + p[8].dst; w.v3b = D + p[9].dst;
+  w.e1 = L(10); w.e2 = L(12); w.e3 = L(14); w.code = D + p[16].dst;
+  w.pe = L(17); w.ze = L(19); w.d1 = L(21); w.d2 = L(23); w.d3 = L(25);
+  w.logstd = D + p[27].dst;
   if (cudaFuncSetAttribute(pmc_policy_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess) {
-    cudaFree(h->d_w); delete h; return fail(LLQ_ECUDA, "cannot reserve shared memory for the policy kernel");
+    release(h); return fail(LLQ_ECUDA, "cannot reserve shared memory for the policy kernel");
   }
   *out = h;
   return LLQ_OK;
 }
 
+int llq_policy_set_weights(llq_policy_handle h, const float* weights, int64_t n_weights, int32_t on_device, void* stream) {
+  if (!h || !weights) return fail(LLQ_EINVAL, "null argument");
+  if (n_weights != LLQ_POLICY_N_WEIGHTS) return fail(LLQ_EINVAL, "weight blob has the wrong length (include/llq_policy.h)");
+  if (on_device != 0 && on_device != 1) return fail(LLQ_EINVAL, "on_device must be 0 (host memory) or 1 (device memory)");
+  if (cudaSetDevice(h->device) != cudaSuccess) return fail(LLQ_ECUDA, "cudaSetDevice failed");
+  const cudaStream_t s = (cudaStream_t)stream;
+  const size_t bytes = sizeof(float) * LLQ_POLICY_N_WEIGHTS;
+  if (on_device) {
+    cudaPointerAttributes a{};
+    if (cudaPointerGetAttributes(&a, weights) != cudaSuccess || a.type != cudaMemoryTypeDevice || a.device != h->device) {
+      cudaGetLastError();
+      return fail(LLQ_EINVAL, "on_device = 1 needs device memory on the handle's device");
+    }
+    return pack(h, weights, s);                // straight from the caller's blob
+  }
+  if (!h->h_stage && (cudaHostAlloc(&h->h_stage, bytes, cudaHostAllocDefault) != cudaSuccess ||
+                      cudaEventCreateWithFlags(&h->ev_stage, cudaEventDisableTiming) != cudaSuccess))
+    return fail(LLQ_ECUDA, "cannot allocate the pinned staging buffer");
+  // the previous host refresh's copy must have left the staging buffer before it is overwritten: the only host wait
+  if (h->staged && cudaEventSynchronize(h->ev_stage) != cudaSuccess) return fail(LLQ_ECUDA, "staging event failed");
+  memcpy(h->h_stage, weights, bytes);
+  if (cudaMemcpyAsync(h->d_raw, h->h_stage, bytes, cudaMemcpyHostToDevice, s) != cudaSuccess ||
+      cudaEventRecord(h->ev_stage, s) != cudaSuccess)
+    return fail(LLQ_ECUDA, "weight upload failed");
+  h->staged = true;
+  return pack(h, h->d_raw, s);
+}
+
 int llq_policy_destroy(llq_policy_handle h) {
   if (!h) return LLQ_OK;
   cudaSetDevice(h->device);
-  cudaFree(h->d_w);
-  delete h;
+  release(h);
   return LLQ_OK;
 }
 

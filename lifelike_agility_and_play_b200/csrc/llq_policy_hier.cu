@@ -20,10 +20,16 @@
 // every thread of a layer reading consecutive columns and using each weight for all 8 rows; 0.23 M MAC per row on the CUDA cores.
 // The recurrent states live in device memory next to the engine's arrays and are wiped where the `done` flag of the previous
 // step is set.
+//
+// Model refresh (llq_hier_policy_set_weights, llq_hier_policy_set_pool_model): the blob is kept as given and the role tables hold
+// offsets into it, so new weights of the same layout are one asynchronous copy on the caller's stream (a pool: into one model's region);
+// the kernels are not involved.
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstdint>
+#include <cstring>
 #include <string>
 #include <vector>
 
@@ -592,11 +598,20 @@ struct llq_hier_policy {
   int device = 0, strategic = 0, train = 0;
   bool attr_set = false;
   float* d_w = nullptr;
+  int64_t n_weights = 0;                                     // the blob's length, fixed at create
   int* d_off = nullptr;
   // pool handles (llq_hier_policy_create_pool): K models, the cutoffs of the next draws, the assign kernel's workspace
   int n_models = 0, max_rows = 0;
   Cutoffs cut{};
   int* d_seg = nullptr;                                      // [K + 1] first CTA of every segment, then the segments' row ids
+  // model k of a pool owns the blob floats [region[k], region_end[k]) (pool_regions); regions_ok = false: two models share arrays
+  std::vector<int64_t> region, region_end;
+  bool regions_ok = false;
+  // host refreshes: pinned staging (stage_len floats), its upload followed by ev_stage
+  float* h_stage = nullptr;
+  int64_t stage_len = 0;
+  cudaEvent_t ev_stage = nullptr;
+  bool staged = false;
 };
 
 namespace {
@@ -610,7 +625,7 @@ int upload(const float* weights, int64_t n_weights, const std::vector<int>& off,
   if (cudaSetDevice(device) != cudaSuccess) return fail_h(LLQ_ECUDA, "cudaSetDevice failed");
   llq_hier_policy* h = new (std::nothrow) llq_hier_policy();
   if (!h) return fail_h(LLQ_ENOMEM, "out of memory");
-  h->device = device; h->strategic = strategic ? 1 : 0; h->train = train;
+  h->device = device; h->strategic = strategic ? 1 : 0; h->train = train; h->n_weights = n_weights;
   if (cudaMalloc(&h->d_w, sizeof(float) * (size_t)n_weights) != cudaSuccess || cudaMalloc(&h->d_off, sizeof(int) * off.size()) != cudaSuccess ||
       cudaMemcpy(h->d_w, weights, sizeof(float) * (size_t)n_weights, cudaMemcpyHostToDevice) != cudaSuccess ||
       cudaMemcpy(h->d_off, off.data(), sizeof(int) * off.size(), cudaMemcpyHostToDevice) != cudaSuccess) {
@@ -645,6 +660,58 @@ Cutoffs cutoffs(const double* probs, int K) {
   for (int k = 0; k < K - 1; k++) c.t[k] = (unsigned long long)std::floor(cum[k] / s * 4294967296.0);
   c.t[K - 1] = 1ull << 32;
   return c;
+}
+
+// model k's region of a pool blob: from its smallest role offset to the next larger model start (or the blob's end); false when two models
+// start at the same float or one of model k's arrays starts outside its region (two models sharing arrays)
+bool pool_regions(const int32_t* offsets, int K, int64_t n_weights, std::vector<int64_t>& lo, std::vector<int64_t>& hi) {
+  lo.assign(K, 0); hi.assign(K, n_weights);
+  for (int k = 0; k < K; k++) {
+    lo[k] = offsets[(size_t)k * RV];
+    for (int r = 1; r < RV; r++) lo[k] = std::min<int64_t>(lo[k], offsets[(size_t)k * RV + r]);
+  }
+  for (int k = 0; k < K; k++)
+    for (int j = 0; j < K; j++) {
+      if (j != k && lo[j] == lo[k]) return false;
+      if (lo[j] > lo[k]) hi[k] = std::min(hi[k], lo[j]);
+    }
+  for (int k = 0; k < K; k++)
+    for (int r = 0; r < RV; r++)
+      if (offsets[(size_t)k * RV + r] >= hi[k]) return false;
+  return true;
+}
+
+// copies n floats of `weights` (host: through the handle's pinned staging; device: checked to lie on the handle's device) to the blob at
+// float `dst`, on `stream`
+int refresh(llq_hier_policy_handle h, int64_t dst, const float* weights, int64_t n, int32_t on_device, void* stream) {
+  if (on_device != 0 && on_device != 1) return fail_h(LLQ_EINVAL, "on_device must be 0 (host memory) or 1 (device memory)");
+  if (cudaSetDevice(h->device) != cudaSuccess) return fail_h(LLQ_ECUDA, "cudaSetDevice failed");
+  const cudaStream_t s = (cudaStream_t)stream;
+  const size_t bytes = sizeof(float) * (size_t)n;
+  if (on_device) {
+    cudaPointerAttributes a{};
+    if (cudaPointerGetAttributes(&a, weights) != cudaSuccess || a.type != cudaMemoryTypeDevice || a.device != h->device) {
+      cudaGetLastError();
+      return fail_h(LLQ_EINVAL, "on_device = 1 needs device memory on the handle's device");
+    }
+    if (cudaMemcpyAsync(h->d_w + dst, weights, bytes, cudaMemcpyDeviceToDevice, s) != cudaSuccess) return fail_h(LLQ_ECUDA, "weight copy failed");
+    return LLQ_OK;
+  }
+  if (h->stage_len < n) {                                    // the first host refresh (a pool's regions may differ in length)
+    if (h->staged && cudaEventSynchronize(h->ev_stage) != cudaSuccess) return fail_h(LLQ_ECUDA, "staging event failed");
+    if (h->h_stage) cudaFreeHost(h->h_stage);
+    h->h_stage = nullptr; h->stage_len = 0; h->staged = false;
+    if (cudaHostAlloc(&h->h_stage, bytes, cudaHostAllocDefault) != cudaSuccess) return fail_h(LLQ_ECUDA, "cannot allocate the pinned staging buffer");
+    h->stage_len = n;
+  }
+  if (!h->ev_stage && cudaEventCreateWithFlags(&h->ev_stage, cudaEventDisableTiming) != cudaSuccess) return fail_h(LLQ_ECUDA, "cudaEventCreate failed");
+  // the previous host refresh's copy must have left the staging buffer before it is overwritten: the only host wait
+  if (h->staged && cudaEventSynchronize(h->ev_stage) != cudaSuccess) return fail_h(LLQ_ECUDA, "staging event failed");
+  memcpy(h->h_stage, weights, bytes);
+  if (cudaMemcpyAsync(h->d_w + dst, h->h_stage, bytes, cudaMemcpyHostToDevice, s) != cudaSuccess || cudaEventRecord(h->ev_stage, s) != cudaSuccess)
+    return fail_h(LLQ_ECUDA, "weight upload failed");
+  h->staged = true;
+  return LLQ_OK;
 }
 
 template <int MODE>
@@ -695,6 +762,8 @@ int llq_hier_policy_destroy(llq_hier_policy_handle h) {
   if (!h) return LLQ_OK;
   cudaSetDevice(h->device);
   cudaFree(h->d_w); cudaFree(h->d_off); cudaFree(h->d_seg);
+  if (h->h_stage) cudaFreeHost(h->h_stage);
+  if (h->ev_stage) cudaEventDestroy(h->ev_stage);
   delete h;
   return LLQ_OK;
 }
@@ -745,6 +814,7 @@ int llq_hier_policy_create_pool(const float* weights, int64_t n_weights, const i
   const int rc = upload(weights, n_weights, off, 1, 0, device, &h);
   if (rc != LLQ_OK) return rc;
   h->n_models = n_models; h->max_rows = max_rows;
+  h->regions_ok = pool_regions(offsets, n_models, n_weights, h->region, h->region_end);
   const std::vector<double> uniform(n_models, 1.0);
   h->cut = cutoffs(uniform.data(), n_models);
   const size_t ws = (size_t)n_models + 1 + ((size_t)(max_rows + kRows - 1) / kRows + n_models) * kRows;
@@ -796,6 +866,23 @@ int llq_hier_policy_forward_pool(llq_hier_policy_handle h, const float* d_obs, i
                                                                                                       d_heading);
   if (cudaGetLastError() != cudaSuccess) return fail_h(LLQ_ECUDA, "hier_pool_kernel launch failed");
   return LLQ_OK;
+}
+
+int llq_hier_policy_set_weights(llq_hier_policy_handle h, const float* weights, int64_t n_weights, int32_t on_device, void* stream) {
+  if (!h || !weights) return fail_h(LLQ_EINVAL, "null argument");
+  if (h->n_models) return fail_h(LLQ_EINVAL, "a pool handle replaces one model at a time: llq_hier_policy_set_pool_model");
+  if (n_weights != h->n_weights) return fail_h(LLQ_EINVAL, "weight blob length differs from the one given at create");
+  return refresh(h, 0, weights, n_weights, on_device, stream);
+}
+
+int llq_hier_policy_set_pool_model(llq_hier_policy_handle h, int32_t k, const float* weights, int64_t n_weights, int32_t on_device,
+                                   void* stream) {
+  if (!h || !weights) return fail_h(LLQ_EINVAL, "null argument");
+  if (!h->n_models) return fail_h(LLQ_EINVAL, "not a pool handle (llq_hier_policy_create_pool)");
+  if (k < 0 || k >= h->n_models) return fail_h(LLQ_EINVAL, "model index outside [0, n_models)");
+  if (!h->regions_ok) return fail_h(LLQ_EINVAL, "the pool's models share arrays: a model has no region of its own");
+  if (n_weights != h->region_end[k] - h->region[k]) return fail_h(LLQ_EINVAL, "weight blob length differs from model k's region");
+  return refresh(h, h->region[k], weights, n_weights, on_device, stream);
 }
 
 const char* llq_hier_policy_last_error(void) { return g_err_h.c_str(); }

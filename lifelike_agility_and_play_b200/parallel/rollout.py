@@ -24,6 +24,10 @@ conversion overlaps the stepping) and carries observation T over to row 0 of the
     - device-side copies interleave both seats' actions into the engine's [2P, 12] action array and put both seats' codes into the code
       column; after the fused step the pair's done flags (equal on both rows) are copied into each seat's contiguous mask for the next
       forwards.
+Model refresh: `update_policy(weights)` (every worker) and `SepmcRolloutWorker.update_opponent(weights, k)` queue the new weights on the
+worker's stream (set_weights / set_model of the handle: a host list, or a flat CUDA tensor, e.g. the blob the learner rank broadcast);
+they take effect from the next `step()`, and the LSTM states, masks, counters and slabs stay as they are: an episode in progress continues
+with the new weights.
 The recurrent levels keep their LSTM states on the device ([N, 128] at the environmental level: code LSTM, then value LSTM; [P, 192]
 for seat 0 at the strategic level: heading, code and value LSTM, and [P, 128] for seat 1), and each forward receives the done flags of
 the step before it, so a finished episode's state is wiped exactly where the reference actor's mask is set.
@@ -116,6 +120,18 @@ class _SlabWorker:
         """Make torch's current stream wait for everything queued so far (call before reading a finished slab there)."""
         torch.cuda.current_stream(self.dev).wait_stream(self.stream)
 
+    def update_policy(self, weights):
+        """The learner's new weights for the worker's policy from the next `step()` on: the refresh is queued on the worker's stream
+        behind every step queued so far (and behind torch's current stream, where a device blob may just have been broadcast).  `weights`:
+        what the policy's `set_weights` takes, the model's arrays or a flat CUDA tensor.  The LSTM states, masks, counters and slabs stay:
+        episodes in progress continue with the new weights.  A refresh between `finish_unroll()` and the next `step()` leaves the finished
+        unroll's bootstrap V computed with the old weights."""
+        self._refresh(self.pol.set_weights, weights)
+
+    def _refresh(self, set_weights, weights, *head):
+        self.stream.wait_stream(torch.cuda.current_stream(self.dev))
+        set_weights(*head, weights, stream=self.stream.cuda_stream)
+
 
 class RolloutWorker(_SlabWorker):
     """The primitive level (PMC, 207-wide observations, `[T+1, N, 223]` slabs).  `finish_unroll()` returns the copy-free `[T, N, 223]`
@@ -169,7 +185,8 @@ class _RecurrentWorker(_SlabWorker):
 
     def _bootstrap(self, obs_row, out):
         # the training forward on a scratch copy of the state with the current counter, so neither the worker's state nor its counter
-        # advances and the next unroll's first forward computes the same V bit for bit
+        # advances and the next unroll's first forward computes the same V bit for bit -- unless update_policy() comes between
+        # finish_unroll() and that forward: the bootstrap keeps the old weights' V, the next forward has the new weights'
         self._scratch_state.copy_(self.state)
         self._forward(obs_row, self._scratch_state, self._scratch_act, 1, values=out.data_ptr())
 
@@ -263,6 +280,19 @@ class SepmcRolloutWorker(_RecurrentWorker):
         super().step()
         with torch.cuda.stream(self.stream):
             self.masks.copy_(self.done.view(self.rows, 2).t())
+
+    def update_opponent(self, weights, k=None):
+        """New weights for the frozen opponent from the next `step()` on, queued like `update_policy`: the single opponent's (`k` None) or
+        model `k` of the opponent pool (`k` required).  `weights`: a strategic-level model (152 arrays) or a flat CUDA tensor in the blob
+        layout.  Pairs in a game against the replaced model continue that game with the new weights and the state they carry."""
+        if self.pool:
+            if k is None:
+                raise ValueError("the worker plays an opponent pool: name the model k to replace")
+            self._refresh(self.opp.set_model, weights, k)
+        else:
+            if k is not None:
+                raise ValueError("the worker plays a single opponent: k must be None")
+            self._refresh(self.opp.set_weights, weights)
 
     def set_opponent_probs(self, probs):
         """The opponent pool's draw probabilities (one per model, >= 0, positive sum) for the games that start from the next step on."""

@@ -73,8 +73,46 @@ POLICY_LIB_PATH = _os.path.join(_os.path.dirname(_os.path.abspath(__file__)), "c
 POLICY_EXPORTS = ["llq_policy_create", "llq_policy_destroy", "llq_policy_forward", "llq_policy_forward_ex", "llq_policy_forward_rec",
                   "llq_policy_last_error", "llq_hier_policy_create", "llq_hier_policy_destroy", "llq_hier_policy_forward",
                   "llq_hier_policy_last_error", "llq_hier_policy_create_train", "llq_hier_policy_forward_rec",
-                  "llq_hier_policy_create_pool", "llq_hier_policy_set_pool_probs", "llq_hier_policy_forward_pool"]
+                  "llq_hier_policy_create_pool", "llq_hier_policy_set_pool_probs", "llq_hier_policy_forward_pool",
+                  "llq_policy_set_weights", "llq_hier_policy_set_weights", "llq_hier_policy_set_pool_model"]
 N_WEIGHTS = 358647
+# array shapes of a shipped primitive-level *.model file, in their stored order (the 28 arrays of include/llq_policy.h)
+PMC_SHAPES = [(1, 135), (1, 135), (1, 72), (1, 72), (207, 256), (256,), (256, 256), (256,), (256, 1), (1,), (207, 256), (256,), (256, 256),
+              (256,), (256, 32), (32,), (32, 256), (135, 64), (64,), (32, 32), (32,), (96, 256), (256,), (256, 256), (256,), (256, 12), (12,),
+              (1, 12)]
+
+
+def check_arrays(weights, shapes, what):
+    """ValueError unless `weights` is a list of len(shapes) arrays of these shapes (unit axes aside: (1, 135) and (135,) agree)."""
+    if isinstance(weights, np.ndarray) or not hasattr(weights, "__len__") or len(weights) != len(shapes):
+        raise ValueError("expected the %d arrays of %s, got %s" % (len(shapes), what, len(weights) if hasattr(weights, "__len__") else type(weights)))
+    for i, (a, want) in enumerate(zip(weights, shapes)):
+        got = np.shape(a)
+        if tuple(d for d in got if d != 1) != tuple(d for d in want if d != 1):
+            raise ValueError("array %d of %s has shape %s, expected %s" % (i, what, got, tuple(want)))
+
+
+def check_device_blob(t, n, device):
+    """ValueError unless `t` is a contiguous 1-D float32 CUDA tensor of `n` floats on cuda:`device`."""
+    import torch
+    if not (isinstance(t, torch.Tensor) and t.is_cuda):
+        raise ValueError("a device weight blob must be a CUDA tensor")
+    if t.dtype != torch.float32 or t.dim() != 1 or not t.is_contiguous() or t.numel() != n:
+        raise ValueError("a device weight blob must be a contiguous 1-D float32 tensor of %d floats (got %s %s)" % (n, t.dtype, tuple(t.shape)))
+    if t.device.index != device:
+        raise ValueError("the weight blob is on %s, the handle on cuda:%d" % (t.device, device))
+
+
+def is_tensor(x):
+    return type(x).__module__.startswith("torch") and hasattr(x, "data_ptr")
+
+
+def keep_for_stream(t, stream, device):
+    """The caching allocator must not hand `t`'s memory out again before the work queued on `stream` (a cudaStream_t, None / 0 = the
+    default stream) has read it."""
+    import torch
+    s = torch.cuda.ExternalStream(stream, device=device) if stream else torch.cuda.default_stream(device)
+    t.record_stream(s)
 
 
 def pack_weights(weights):
@@ -101,6 +139,7 @@ class DevicePolicy:
         L.llq_policy_destroy.argtypes = [_C.c_void_p]
         L.llq_policy_last_error.restype = _C.c_char_p
         blob = pack_weights(weights)
+        self.device = int(device)
         self._h = _C.c_void_p()
         rc = L.llq_policy_create(blob.ctypes.data_as(_C.c_void_p), blob.size, device, _C.byref(self._h))
         if rc != 0:
@@ -127,6 +166,26 @@ class DevicePolicy:
                                               seed, counter, row_gid0, stream)
         if rc != 0:
             raise RuntimeError("llq_policy_forward_rec failed (%d): %s" % (rc, (self._lib.llq_policy_last_error() or b"").decode()))
+
+    def set_weights(self, weights, stream=None):
+        """The learner's new weights (include/llq_policy.h, llq_policy_set_weights), asynchronous on `stream` (a cudaStream_t, None = the
+        default stream): forwards queued there before see the old weights, forwards queued after it the new ones.  `weights`: the 28
+        arrays of a model file (the host list may be reused as soon as this returns), or a flat float32 CUDA tensor of N_WEIGHTS floats
+        on the handle's device (pack_weights' layout)."""
+        if is_tensor(weights):
+            check_device_blob(weights, N_WEIGHTS, self.device)
+            ptr, on_device = weights.data_ptr(), 1
+        else:
+            check_arrays(weights, PMC_SHAPES, "a primitive-level model")
+            blob = pack_weights(weights)
+            ptr, on_device = blob.ctypes.data, 0
+        L = self._lib
+        L.llq_policy_set_weights.argtypes = [_C.c_void_p, _C.c_void_p, _C.c_int64, _C.c_int32, _C.c_void_p]
+        rc = L.llq_policy_set_weights(self._h, ptr, N_WEIGHTS, on_device, stream)
+        if rc != 0:
+            raise RuntimeError("llq_policy_set_weights failed (%d): %s" % (rc, (L.llq_policy_last_error() or b"").decode()))
+        if on_device:
+            keep_for_stream(weights, stream, self.device)
 
     def close(self):
         if getattr(self, "_h", None):

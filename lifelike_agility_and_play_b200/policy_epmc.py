@@ -29,6 +29,8 @@ import ctypes as C
 
 import numpy as np
 
+from .policy import check_arrays, check_device_blob, is_tensor, keep_for_stream
+
 
 def _same_pad(n, k, s):
     out = -(-n // s)
@@ -371,8 +373,10 @@ def _policy_lib():
     return lib
 
 
-def _weight_blob(weights):
-    """(blob, starts): the arrays concatenated as fp32, each starting on a 16-byte boundary (the kernel's float4 loads)."""
+def weight_blob(weights):
+    """(blob, starts): the arrays concatenated as fp32, each starting on a 16-byte boundary (the kernel's float4 loads).  The one builder
+    of the layout the device handles keep: a learner forms the blob it broadcasts to its actors with it (blob as a CUDA tensor goes to
+    `set_weights` / `DeviceOpponentPool.set_model`)."""
     w = [np.ascontiguousarray(a, np.float32).reshape(-1) for a in weights]
     w = [np.concatenate([a, np.zeros((-a.size) % 4, np.float32)]) for a in w]
     starts = np.concatenate([[0], np.cumsum([a.size for a in w])]).astype(np.int64)
@@ -380,17 +384,31 @@ def _weight_blob(weights):
 
 
 def _blob_and_tables(models, *roles):
-    """(blob, tables): the arrays of all `models` in one fp32 blob, model after model (each laid out by `_weight_blob`), and for each list
+    """(blob, tables): the arrays of all `models` in one fp32 blob, model after model (each laid out by `weight_blob`), and for each list
     of array indices in `roles` the int32 table of where those arrays start in the blob, model after model (the role tables of
     include/llq_policy.h)."""
     blobs, starts, base = [], [], 0
     for m in models:
-        blob, s = _weight_blob(m)
+        blob, s = weight_blob(m)
         blobs.append(blob)
         starts.append(s + base)
         base += blob.size
     blob = np.concatenate(blobs) if blobs else np.zeros(0, np.float32)
     return blob, [np.array([s[i] for s in starts for i in r], np.int32) for r in roles]
+
+
+def pool_regions(offsets, n_models, n_weights):
+    """[(lo, hi)] per model of a pool blob (include/llq_policy.h, llq_hier_policy_set_pool_model): model k's region runs from its smallest
+    role offset to the next larger model start, or to the end of the blob; None when two models share arrays (two models starting at
+    the same float, or one of model k's arrays starting outside its region).  `offsets`: the pool's [n_models * 101] role table."""
+    off = np.asarray(offsets, np.int64).reshape(n_models, -1)
+    lo = off.min(1)
+    if len(set(lo.tolist())) < n_models:
+        return None
+    hi = [min([int(x) for x in lo if x > lo[k]], default=int(n_weights)) for k in range(n_models)]
+    if any((off[k] >= hi[k]).any() for k in range(n_models)):
+        return None
+    return [(int(lo[k]), hi[k]) for k in range(n_models)]
 
 
 def _vp(a):
@@ -412,6 +430,30 @@ class _HierHandle:
         if getattr(self.lib, entry)(*args):
             raise error("%s: %s" % (entry, self.lib.llq_hier_policy_last_error().decode()))
 
+    def _refresh(self, entry, head, weights, n, shapes, what, stream):
+        """`entry`(*head, weights, n, on_device, stream): the checks of a host list (the level's `shapes`) or a flat CUDA tensor of n floats,
+        then the library call; a device source is kept from the allocator until the copy on `stream` has run."""
+        if is_tensor(weights):
+            check_device_blob(weights, n, self.device)
+            ptr, on_device = weights.data_ptr(), 1
+        else:
+            check_arrays(weights, shapes, what)
+            blob = weight_blob(weights)[0]
+            if blob.size != n:
+                raise ValueError("the blob of %s has %d floats, the handle expects %d" % (what, blob.size, n))
+            ptr, on_device = blob.ctypes.data, 0
+        self._call(entry, *head, C.c_void_p(ptr), C.c_int64(n), C.c_int32(on_device), C.c_void_p(stream or 0))
+        if on_device:
+            keep_for_stream(weights, stream, self.device)
+
+    def set_weights(self, weights, stream=None):
+        """The learner's new weights (include/llq_policy.h, llq_hier_policy_set_weights), asynchronous on `stream` (a cudaStream_t, None =
+        the default stream): forwards queued there before see the old weights, forwards queued after it the new ones; the LSTM states
+        are the caller's and stay.  `weights`: the level's arrays (102 / 152; the host list may be reused as soon as this returns), or a
+        flat float32 CUDA tensor on the handle's device in the blob layout (`weight_blob(arrays)[0]`)."""
+        self._refresh("llq_hier_policy_set_weights", (self._h,), weights, self.n_weights, SEPMC_SHAPES if self.strategic else EPMC_SHAPES,
+                      "a strategic-level model" if self.strategic else "an environmental-level model", stream)
+
     def close(self):
         if self._h:
             self.lib.llq_hier_policy_destroy(self._h)
@@ -426,7 +468,7 @@ class DeviceHierPolicy(_HierHandle):
 
     def __init__(self, weights, device=0, train=False):
         assert len(weights) in (102, 152), "expected an environmental-level (102 arrays) or a strategic-level (152 arrays) model"
-        self.strategic, self.train = len(weights) == 152, bool(train)
+        self.strategic, self.train, self.device = len(weights) == 152, bool(train), int(device)
         if self.train:
             blob, (off, voff) = _blob_and_tables([weights], hier_role_arrays(self.strategic), hier_role_arrays(False, value_tower=True))
             super().__init__("llq_hier_policy_create_train", _vp(blob), C.c_int64(blob.size), _vp(off), C.c_int32(off.size), _vp(voff),
@@ -435,6 +477,7 @@ class DeviceHierPolicy(_HierHandle):
             blob, (off,) = _blob_and_tables([weights], hier_role_arrays(self.strategic))
             super().__init__("llq_hier_policy_create", _vp(blob), C.c_int64(blob.size), _vp(off), C.c_int32(off.size),
                              C.c_int32(int(self.strategic)), C.c_int32(device))
+        self.n_weights = blob.size
         self.state_dim = 128 if (self.strategic or self.train) else 64
         self.obs_dim = 965 if self.strategic else 916
 
@@ -458,10 +501,11 @@ class DeviceSepmcTrainPolicy(_HierHandle):
 
     def __init__(self, weights, device=0):
         assert len(weights) == 152, "expected a strategic-level model (152 arrays)"
-        self.strategic, self.train = True, True
+        self.strategic, self.train, self.device = True, True, int(device)
         blob, (off, toff) = _blob_and_tables([weights], hier_role_arrays(True), strategic_train_role_arrays())
         super().__init__("llq_hier_policy_create_train_strategic", _vp(blob), C.c_int64(blob.size), _vp(off), C.c_int32(off.size), _vp(toff),
                          C.c_int32(toff.size), C.c_int32(device))
+        self.n_weights = blob.size
         self.state_dim, self.obs_dim = 192, 965
 
     # the deterministic entry, which the library refuses for this handle: `forward` raises the library's RuntimeError (naming
@@ -486,14 +530,31 @@ class DeviceOpponentPool(_HierHandle):
 
     def __init__(self, models, device=0, *, max_rows, probs=None):
         assert all(len(m) == 152 for m in models), "expected strategic-level models (152 arrays)"
-        self.strategic, self.train = True, False
+        self.strategic, self.train, self.device = True, False, int(device)
         self.n_models, self.max_rows = len(models), int(max_rows)
         self.state_dim, self.obs_dim = 128, 965
         blob, (off,) = _blob_and_tables(models, hier_role_arrays(True))
         super().__init__("llq_hier_policy_create_pool", _vp(blob), C.c_int64(blob.size), _vp(off), C.c_int32(self.n_models), C.c_int32(self.max_rows),
                          C.c_int32(device))
+        self.n_weights, self.regions = blob.size, pool_regions(off, self.n_models, blob.size)
         if probs is not None:
             self.set_probs(probs)
+
+    def set_weights(self, weights, stream=None):
+        raise ValueError("a pool replaces one model at a time: set_model(k, weights)")
+
+    def set_model(self, k, weights, stream=None):
+        """Replaces model k (include/llq_policy.h, llq_hier_policy_set_pool_model), asynchronous on `stream` as `set_weights` is; the
+        number of models stays.  `weights`: a strategic-level model (152 arrays), or a flat float32 CUDA tensor on the handle's device
+        holding `weight_blob(arrays)[0]`.  Pairs whose current game is against model k continue it with the new weights and the state
+        they carry; a model with probability 0 can be filled here and given a probability later (`set_probs`)."""
+        if not 0 <= int(k) < self.n_models:
+            raise ValueError("model index %s outside [0, %d)" % (k, self.n_models))
+        if self.regions is None:
+            raise ValueError("the pool's models share arrays: no model has a region of its own")
+        lo, hi = self.regions[int(k)]
+        self._refresh("llq_hier_policy_set_pool_model", (self._h, C.c_int32(int(k))), weights, hi - lo, SEPMC_SHAPES, "a strategic-level model",
+                      stream)
 
     def set_probs(self, probs):
         """Draw probabilities of the next forwards: one finite entry >= 0 per model, positive sum (they need not sum to 1)."""
