@@ -35,17 +35,71 @@ constexpr int kMaxSph = 32, kMaxCon = 8, kMaxLim = 8;
 struct SphConst { float c[3]; float r; float mu_link; int leg; int depth; int foot; };   // centre in the frame of link (leg, depth - 1); depth 0 = base
 struct alignas(16) SphTable { int n; int rule; int pad[2]; SphConst s[kMaxSph]; };         // rule: llq_config.knee_contacts
 
-// per-env shared-memory tables (floats)
-constexpr int kLinkTab = 12 * 8;      // link (3 k + i): c1 s1 cy sy | p(3) | -
-constexpr int kLegTab = 4 * 48;       // leg k: dynamics phase F(18) Hrow(9) rhs(3) Ic(10) facc(6); rows phase W(18) L(3) dinv(3) qd(3)
-constexpr int kConW = 20, kConTab = kMaxCon * kConW;   // contact: leg depth | Pc(3) n(3) t1(3) t2(3) | dist mu lam0 lam | - -
-                                                       // (during the friction pass: ... lam0 | mu lam_n | lam_t1 lam_t2)
-constexpr int kLimTab = kMaxLim * 4;  // limit row: leg joint dir pen
-constexpr int kRowW = 12, kRowTab = 32 * kRowW;        // row: y(6) e(3) leg - -   (aliased by the 16 x 20 float scratch of the dynamics phase)
-constexpr int kEnvTab = 56;           // p_base(6) - - | Cholesky factor of the base block (21) - - - | joint targets (12) | actions (12)
+// Per-env shared-memory tables, at kLinkOff ... kEnvOff from the env's base s_env_dyn + e * kEnvFloats.  A table is a run of records;
+// the slot names are offsets in one record (ints are stored as their bits).  Where a table changes meaning during a sub-step, each
+// phase has its own names on the same offsets.
+// link record 3 k + i (body i of leg k): rotation Rx(c1, s1) Ry(cy, sy) and origin p of the body, base coordinates
+constexpr int kLinkW = 8, kLinkTab = 12 * kLinkW;
+constexpr int kLkC1 = 0, kLkS1 = 1, kLkCy = 2, kLkSy = 3, kLkP = 4;
+// leg record k, dynamics phase: the leg's blocks of the mass matrix and what its composite rigid body carries
+constexpr int kLegW = 48, kLegTab = 4 * kLegW;
+constexpr int kLgF = 0;                                  // coupling block F_k: one 6-vector per joint
+constexpr int kLgH = 18;                                 // joint-space inertia H_k, row major (9)
+constexpr int kLgRhs = 27;                               // tau - C per joint (3)
+constexpr int kLgMass = 30, kLgMom = 31, kLgI = 34;      // the leg as one body: mass, first moment (3), inertia (Sym3 order, 6)
+constexpr int kLgBias = 40;                              // accumulated bias wrench of the leg (6)
+// leg record k, rows phase (from the __syncwarp that ends the dynamics): the factorised leg and its predicted joint velocities
+constexpr int kLgW = 0;                                  // W = F L^-T: one 6-vector per joint
+constexpr int kLgL10 = 18, kLgL20 = 19, kLgL21 = 20;     // H_k = L D L^T
+constexpr int kLgDinv = 21, kLgQd = 24;                  // D^-1 (3), predicted joint velocities (3)
+constexpr int kLgC3 = 28, kLgS3 = 29;                    // knee cosine and sine (fp64 centres of the shank's spheres)
+// contact record, one per manifold point
+constexpr int kConW = 20, kConTab = kMaxCon * kConW;
+constexpr int kCoLeg = 0, kCoDepth = 1;                  // leg of the sphere's link (-1: the base), depth of the link (int bits)
+constexpr int kCoPc = 2;                                 // contact point (3)
+constexpr int kCoDir = 5;                                // row directions, 3 each: normal, tangents t1, t2 (row d at kCoDir + 3 d)
+constexpr int kCoDist = 14, kCoMu = 15, kCoLam0 = 16;    // signed distance, friction coefficient, warm start of the normal impulse
+constexpr int kCoLam = 17;                               // normal impulse after the solve (the next sub-step's warm start)
+constexpr int kCoCone = 17, kCoLamT1 = 18, kCoLamT2 = 19;   // during a friction pass: mu lam_n, impulses of the two tangent rows
+// limit record, one per violated joint limit
+constexpr int kLimW = 4, kLimTab = kMaxLim * kLimW;
+constexpr int kLmLeg = 0, kLmJoint = 1, kLmDir = 2, kLmPen = 3;   // leg, joint (int bits), direction +-1, penetration
+// row record, one per constraint row: its image under the factorised mass matrix, for the other rows' Delassus entries
+constexpr int kRowW = 12, kRowTab = 32 * kRowW;
+constexpr int kRwY = 0, kRwE = 6, kRwLeg = 9;            // y (6), e = D^-1 w (3), leg (int bits)
+// the row table's other uses: the dynamics' scratch, one record per lane l16 for the suffix sums along a leg ...
+constexpr int kScrW = 20;
+constexpr int kScBias = 0, kScMass = 6, kScMom = 7, kScI = 10;   // bias wrench (6), mass, first moment (3), inertia (6)
+// ... the totals of the env's rows after the sweep (18 floats at its head), and after the last sub-step the TailState
+constexpr int kResBase = 0, kResLeg = 6;                 // sum lam y (6); per leg k, sum lam w at kResLeg + 3 k
+// env record (one per env)
+constexpr int kEnvTab = 56;
+constexpr int kEvBias = 0;                               // dynamics phase: bias wrench of the base body (6)
+constexpr int kEvVel = 0;                                // rows phase: predicted base velocity w, v (base coordinates, 6)
+constexpr int kEvChol = 8;                               // Cholesky factor of the base block (21, packed as in llq_math.cuh)
+constexpr int kEvTarget = 32, kEvAct = 44;               // clipped joint targets (12), actions (12)
 constexpr int kATabWarp = 32 * 32;     // Delassus coefficients of one WARP (its two envs' rows packed into 32 lanes): atab[col * 32 + lane]
 constexpr int kEnvFloats = 944;        // >= the sum of the tables, and = 16 (mod 32): envs an odd number of slots apart hit disjoint banks
-static_assert(kLinkTab + kLegTab + kConTab + kLimTab + kRowTab + kEnvTab <= kEnvFloats && kEnvFloats % 32 == 16, "per-env table layout");
+static_assert(16 * kScrW <= kRowTab && kResLeg + 4 * 3 <= kRowTab, "the row table's other uses fit in it");
+constexpr int kLinkOff = 0, kLegOff = kLinkOff + kLinkTab, kConOff = kLegOff + kLegTab, kLimOff = kConOff + kConTab;
+constexpr int kRowOff = kLimOff + kLimTab, kEnvOff = kRowOff + kRowTab;
+static_assert(kEnvOff + kEnvTab <= kEnvFloats && kEnvFloats % 32 == 16, "per-env table layout");
+// frames of leg k's three bodies from the link table: hip Rx(c1, s1), thigh Ry(c2, s2), shank Ry(c23, s23); origins p1 p2 p3
+struct LegFrames {
+  float c1, s1, c2, s2, c23, s23;
+  V3 p1, p2, p3;
+  LLQ_DI V3 on_thigh(V3 c) const { return p2 + rot<0>(rot<1>(c, c2, s2), c1, s1); }     // base coordinates of a point fixed to the thigh
+  LLQ_DI V3 on_shank(V3 c) const { return p3 + rot<0>(rot<1>(c, c23, s23), c1, s1); }   // ... and to the shank
+};
+LLQ_DI LegFrames leg_frames(const float* link, int k) {
+  const float* lk = link + 3 * k * kLinkW;
+  LegFrames f;
+  f.c1 = lk[kLkC1]; f.s1 = lk[kLkS1];
+  f.c2 = lk[kLinkW + kLkCy]; f.s2 = lk[kLinkW + kLkSy];
+  f.c23 = lk[2 * kLinkW + kLkCy]; f.s23 = lk[2 * kLinkW + kLkSy];
+  f.p1 = ld3(lk + kLkP); f.p2 = ld3(lk + (kLinkW + kLkP)); f.p3 = ld3(lk + (2 * kLinkW + kLkP));
+  return f;
+}
 
 LLQ_DI V3 rotxy(V3 v, float cy, float sy, float cx, float sx) { return rot<0>(rot<1>(v, cy, sy), cx, sx); }     // Rx Ry v
 LLQ_DI V3 rotxyT(V3 v, float cy, float sy, float cx, float sx) { return rotT<1>(rotT<0>(v, cx, sx), cy, sy); }  // (Rx Ry)^T v
@@ -178,12 +232,12 @@ struct RowRegs { float y[6], wj[3], b, rhs, invd, lam, hi, mu; int leg; };
 // row rr of the env behind in.tb: contact rr / 3 in direction rr % 3, or limit row rr - 3 nc; also leaves (y, e = D^-1 w, leg) in the
 // env's row table for the other rows' Delassus entries.  Returns true for a normal row (its impulse is the contact's warm start).
 LLQ_DI bool row_image(const RowsIn& in, RowRegs& r) {
-  const float* linktab = in.tb;
-  const float* legtab = in.tb + kLinkTab;
-  const float* contab = legtab + kLegTab;
-  const float* limtab = contab + kConTab;
-  float* rowtab = in.tb + kLinkTab + kLegTab + kConTab + kLimTab;
-  const float* envtab = rowtab + kRowTab;
+  const float* linktab = in.tb + kLinkOff;
+  const float* legtab = in.tb + kLegOff;
+  const float* contab = in.tb + kConOff;
+  const float* limtab = in.tb + kLimOff;
+  float* rowtab = in.tb + kRowOff;
+  const float* envtab = in.tb + kEnvOff;
   const int rr = in.rr;
   const bool is_con = rr < 3 * in.nc;
   const int d = rr % 3, cq = rr / 3;
@@ -199,41 +253,41 @@ LLQ_DI bool row_image(const RowsIn& in, RowRegs& r) {
     int leg, jj = 0;
     if (is_con) {
       const float* cr = contab + cq * kConW;
-      leg = __float_as_int(cr[0]);
-      const int depth = __float_as_int(cr[1]);
-      const V3 Pc = ld3(cr + 2), dir = ld3(cr + 5 + 3 * d);
-      dist = cr[14]; r.mu = cr[15]; lam0 = cr[16];
+      leg = __float_as_int(cr[kCoLeg]);
+      const int depth = __float_as_int(cr[kCoDepth]);
+      const V3 Pc = ld3(cr + kCoPc), dir = ld3(cr + kCoDir + 3 * d);
+      dist = cr[kCoDist]; r.mu = cr[kCoMu]; lam0 = cr[kCoLam0];
       Ga = cross(Pc, dir); Gl = dir;
-      rel = dot(Ga, ld3(envtab)) + dot(Gl, ld3(envtab + 3));     // predicted base velocity (base coordinates), parked by the env's lane 0
+      rel = dot(Ga, ld3(envtab + kEvVel)) + dot(Gl, ld3(envtab + (kEvVel + 3)));   // parked by the env's lane 0
       if (leg >= 0) {
-        const float* lk = linktab + leg * 24;
-        const float c1 = lk[0], s1 = lk[1];
-        const V3 p1 = ld3(lk + 4), p2 = ld3(lk + 12), p3 = ld3(lk + 20), n2 = V3{0.f, -c1, -s1};
+        const float* lk = linktab + leg * (3 * kLinkW);      // (not leg_frames: with it this block compiles differently)
+        const float c1 = lk[kLkC1], s1 = lk[kLkS1];
+        const V3 p1 = ld3(lk + kLkP), p2 = ld3(lk + (kLinkW + kLkP)), p3 = ld3(lk + (2 * kLinkW + kLkP)), n2 = V3{0.f, -c1, -s1};
         j[0] = Ga.x + dot(cross(p1, V3{1.f, 0.f, 0.f}), Gl);
         if (depth >= 2) j[1] = dot(n2, Ga) + dot(cross(p2, n2), Gl);
         if (depth >= 3) j[2] = dot(n2, Ga) + dot(cross(p3, n2), Gl);
       }
     } else {
-      const float* lr = limtab + (rr - 3 * in.nc) * 4;
-      leg = __float_as_int(lr[0]); jj = __float_as_int(lr[1]); dirl = lr[2]; pen = lr[3];
+      const float* lr = limtab + (rr - 3 * in.nc) * kLimW;
+      leg = __float_as_int(lr[kLmLeg]); jj = __float_as_int(lr[kLmJoint]); dirl = lr[kLmDir]; pen = lr[kLmPen];
       j[0] = jj == 0 ? dirl : 0.f; j[1] = jj == 1 ? dirl : 0.f; j[2] = jj == 2 ? dirl : 0.f;
     }
     r.leg = leg;
     float g[6] = {Ga.x, Ga.y, Ga.z, Gl.x, Gl.y, Gl.z};
     if (leg >= 0) {
-      const float* lt = legtab + leg * 48;
-      const float L10 = lt[18], L20 = lt[19], L21 = lt[20];
-      rel += j[0] * lt[24] + j[1] * lt[25] + j[2] * lt[26];
+      const float* lt = legtab + leg * kLegW;
+      const float L10 = lt[kLgL10], L20 = lt[kLgL20], L21 = lt[kLgL21];
+      rel += j[0] * lt[kLgQd] + j[1] * lt[kLgQd + 1] + j[2] * lt[kLgQd + 2];
       r.wj[0] = j[0];
       r.wj[1] = fmaf(-L10, r.wj[0], j[1]);
       r.wj[2] = fmaf(-L20, r.wj[0], fmaf(-L21, r.wj[1], j[2]));
-      e[0] = r.wj[0] * lt[21]; e[1] = r.wj[1] * lt[22]; e[2] = r.wj[2] * lt[23];
+      e[0] = r.wj[0] * lt[kLgDinv]; e[1] = r.wj[1] * lt[kLgDinv + 1]; e[2] = r.wj[2] * lt[kLgDinv + 2];
 #pragma unroll
       for (int m = 0; m < 3; m++)
 #pragma unroll
-        for (int t = 0; t < 6; t++) g[t] = fmaf(-e[m], lt[6 * m + t], g[t]);
+        for (int t = 0; t < 6; t++) g[t] = fmaf(-e[m], lt[kLgW + 6 * m + t], g[t]);
     }
-    chol6_fwd_p(envtab + 8, g, r.y);
+    chol6_fwd_p(envtab + kEvChol, g, r.y);
     const float dg = dot6(r.y, r.y) + r.wj[0] * e[0] + r.wj[1] * e[1] + r.wj[2] * e[2];
     r.invd = 1.0f / dg;
     if (is_con) {
@@ -252,15 +306,15 @@ LLQ_DI bool row_image(const RowsIn& in, RowRegs& r) {
       r.hi = in.max_imp;
     }
     float* rw = rowtab + rr * kRowW;
-    st4(rw, r.y[0], r.y[1], r.y[2], r.y[3]);
-    st4(rw + 4, r.y[4], r.y[5], e[0], e[1]);
-    st4(rw + 8, e[2], __int_as_float(r.leg), 0.f, 0.f);
+    st4(rw + kRwY, r.y[0], r.y[1], r.y[2], r.y[3]);
+    st4(rw + (kRwY + 4), r.y[4], r.y[5], e[0], e[1]);
+    st4(rw + (kRwE + 2), e[2], __int_as_float(r.leg), 0.f, 0.f);
   }
   return act && is_con && d == 0;
 }
 // entry (r, col) of the Delassus matrix from this lane's row r and the table entry of row `col`
 LLQ_DI float delassus_entry(const RowRegs& r, const float* rw) {
-  const float4 a = ld4(rw), bq = ld4(rw + 4), cq4 = ld4(rw + 8);
+  const float4 a = ld4(rw + kRwY), bq = ld4(rw + (kRwY + 4)), cq4 = ld4(rw + (kRwE + 2));
   const float ys[6] = {a.x, a.y, a.z, a.w, bq.x, bq.y};
   const float jt = r.wj[0] * bq.z + r.wj[1] * bq.w + r.wj[2] * cq4.x;
   return dot6(r.y, ys) + (__float_as_int(cq4.y) == r.leg ? jt : 0.f);
@@ -288,7 +342,7 @@ LLQ_DI void impulse_sums(const RowsIn& in, const RowRegs& r) {
   for (int kk = 0; kk < 4; kk++) {
     const float f = r.leg == kk ? r.lam : 0.f;
 #pragma unroll
-    for (int m = 0; m < 3; m++) v18[6 + 3 * kk + m] = f * r.wj[m];
+    for (int m = 0; m < 3; m++) v18[kResLeg + 3 * kk + m] = f * r.wj[m];
   }
   if (in.split != 16) {                                     // warp-uniform
     const bool foreign = (in.lane >= 16) != (in.lane >= in.split);      // the row belongs to the other half-warp's env
@@ -327,7 +381,7 @@ LLQ_DI void solve_rows(const RowsIn& in) {
   // even (the sweeps are unrolled by two; the caps are even).
   const int Ce = (in.Cmax + 1) & ~1, Le = (in.Lmax + 1) & ~1;
   {
-    const float* rowtab = in.tb + kLinkTab + kLegTab + kConTab + kLimTab;
+    const float* rowtab = in.tb + kRowOff;
     const int ncon = 3 * nc;
 #pragma unroll 1
     for (int col = 0; col < 3 * Ce; col += 2) {     // two columns per iteration (3 Ce and Le are even)
@@ -357,7 +411,7 @@ LLQ_DI void solve_rows(const RowsIn& in) {
   const int d = in.rr % 3;
   const int at_lim = is_lim ? lane : -1, at_nrm = is_normal ? lane : -1;
   const int at_fric = is_con && d != 0 ? lane - d : -1;      // a tangent row commits at its contact's step, whose source lane is the normal's
-  float* const cfric = in.tb + kLinkTab + kLegTab + 16;       // per contact: lam0 | cone radius mu lam_n | impulses of the two tangents
+  float* const cfric = in.tb + (kConOff + kCoLam0);     // per contact: lam0 | kCoCone kCoLamT1 kCoLamT2, one float4
   float rc = r.lam + r.rhs;
 #define LLQ16_CLAMP_LIMIT(x) fminf(fmaxf((x), 0.f), r.hi)      /* joint-limit rows: [0, max impulse] */
 #define LLQ16_CLAMP_NORMAL(x) fmaxf((x), 0.f)                  /* normal rows: [0, 1e10] -- the upper bound never binds a finite state */
@@ -395,7 +449,7 @@ LLQ_DI void solve_rows(const RowsIn& in) {
       // contact records (one float4 per step, off the dependent chain) instead of three shuffles per step.  Records beyond the env's
       // contacts hold finite values of earlier sub-steps (zeros at the start of the kernel).
       __syncwarp();                                           // the previous pass's reads of the records are done
-      if (is_con) cfric[(in.rr / 3) * kConW + 1 + d] = d == 0 ? r.mu * r.lam : r.lam;
+      if (is_con) cfric[(in.rr / 3) * kConW + (kCoCone - kCoLam0) + d] = d == 0 ? r.mu * r.lam : r.lam;
       __syncwarp();
 #pragma unroll 1
       for (int t = 0; t < in.Cmax; t++) {                       // friction pairs with the implicit cone (resolveConeFrictionConstraintRows)
@@ -423,7 +477,7 @@ LLQ_DI void solve_rows(const RowsIn& in) {
 #undef LLQ16_CLAMP_NORMAL
   T16_IN(10);
   // the normal impulses go back to the contact records (warm start of the next sub-step)
-  if (is_normal) in.tb[kLinkTab + kLegTab + (in.rr / 3) * kConW + 17] = r.lam;
+  if (is_normal) in.tb[kConOff + (in.rr / 3) * kConW + kCoLam] = r.lam;
   __syncwarp();                     // every lane is done with the row table: its head becomes the result area
   impulse_sums(in, r);
   T16_IN(3);
@@ -700,15 +754,14 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
   const LegConst& L = M.leg[k];
   const V3 r0 = ld3(L.j[0].r), r1 = ld3(L.j[1].r), r2 = ld3(L.j[2].r);
   float* const linktab = s_env_dyn + el * kEnvFloats;
-  float* const legtab = linktab + kLinkTab;
-  float* const contab = legtab + kLegTab;
-  float* const limtab = contab + kConTab;
-  float* const rowtab = limtab + kLimTab;
-  float* const scr = rowtab;                         // dynamics-phase scratch (16 lanes x 20 floats) aliases the row table
-  float* const envtab = rowtab + kRowTab;
+  float* const legtab = linktab + kLegOff;
+  float* const contab = linktab + kConOff;
+  float* const limtab = linktab + kLimOff;
+  float* const rowtab = linktab + kRowOff;
+  float* const envtab = linktab + kEnvOff;
   float* const s_atab = s_env_dyn + EPB * kEnvFloats;   // [BLOCK / 32][32 cols][32 lanes] Delassus coefficients, one table per warp
   for (int col = 0; col < 32; col++) s_atab[(tid >> 5) * kATabWarp + col * 32 + (tid & 31)] = 0.f;      // finite from the start (masked steps multiply them by 0)
-  for (int t = l16; t < kConTab; t += 16) contab[t] = 0.f;      // so are the contact records the friction sweep reads on its padded steps
+  for (int t = l16; t < kConTab; t += 16) contab[t] = 0.f;     // so are the contact records the friction sweep reads on its padded steps
   // joints with a lower dof index than this lane's (k, i): rank of a violated limit in Bullet's row order
   unsigned lowmask = 0;
 #pragma unroll
@@ -728,8 +781,8 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
   }
   if (i < 3) {                                               // joint (k, i): action and clipped target stay in shared memory
     const float a = actions[(size_t)env * kActDim + 3 * k + i];
-    envtab[44 + 3 * k + i] = a;
-    envtab[32 + 3 * k + i] = clampf((i == 0 ? q[0] : (i == 1 ? q[1] : q[2])) + a, -3.0f, 3.0f);           // PLE:200, LR:126-127
+    envtab[kEvAct + 3 * k + i] = a;
+    envtab[kEvTarget + 3 * k + i] = clampf((i == 0 ? q[0] : (i == 1 ? q[1] : q[2])) + a, -3.0f, 3.0f);           // PLE:200, LR:126-127
   }
   const int nsph = ST.n, rule = ST.rule;
   float warm[2];                                             // remembered normal impulses of spheres l16 and l16 + 16
@@ -872,15 +925,15 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
     }
     // ---------------- composite inertia / accumulated bias wrench along the leg (suffix sums through the scratch rows)
     {
-      float* my = scr + l16 * 20;
-      st4(my, f.a.x, f.a.y, f.a.z, f.l.x); st4(my + 4, f.l.y, f.l.z, mc_, hc.x);
-      st4(my + 8, hc.y, hc.z, Ic.xx, Ic.xy); st4(my + 12, Ic.xz, Ic.yy, Ic.yz, Ic.zz);
+      float* my = rowtab + l16 * kScrW;
+      st4(my + kScBias, f.a.x, f.a.y, f.a.z, f.l.x); st4(my + (kScBias + 4), f.l.y, f.l.z, mc_, hc.x);
+      st4(my + (kScMom + 1), hc.y, hc.z, Ic.xx, Ic.xy); st4(my + (kScI + 2), Ic.xz, Ic.yy, Ic.yz, Ic.zz);
       __syncwarp();
       if (i < 2) {
 #pragma unroll 1
         for (int up = i + 1; up < 3; up++) {
-          const float* o = scr + (k + 4 * up) * 20;
-          const float4 a = ld4(o), b4 = ld4(o + 4), c4 = ld4(o + 8), d4 = ld4(o + 12);
+          const float* o = rowtab + (k + 4 * up) * kScrW;
+          const float4 a = ld4(o + kScBias), b4 = ld4(o + (kScBias + 4)), c4 = ld4(o + (kScMom + 1)), d4 = ld4(o + (kScI + 2));
           f.a = f.a + V3{a.x, a.y, a.z}; f.l = f.l + V3{a.w, b4.x, b4.y};
           mc_ += b4.z; hc = hc + V3{b4.w, c4.x, c4.y};
           Ic = Ic + Sym3{c4.z, c4.w, d4.x, d4.y, d4.z, d4.w};
@@ -894,22 +947,24 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
       const float Cb = dot(ax, f.a) + dot(al, f.l);
       const float h0 = Fa.x + dot(l1, Fl), h1 = dot(n2, Fa) + dot(l2, Fl), h2 = dot(n2, Fa) + dot(l3, Fl);
       const float qi = i == 0 ? q[0] : (i == 1 ? q[1] : q[2]), qdi = i == 0 ? qd[0] : (i == 1 ? qd[1] : qd[2]);
-      const float tg = envtab[32 + 3 * k + ic];
+      const float tg = envtab[kEvTarget + 3 * k + ic];
       const float tau = clampf(fmaf(P.kp, tg - qi, P.kd * (0.f - qdi)), -P.max_tau, P.max_tau) - L.j[ic].jdamp * qdi;
-      float* lt = legtab + k * 48;
+      float* lt = legtab + k * kLegW;
       if (i < 3) {
-        lt[6 * i] = Fa.x; lt[6 * i + 1] = Fa.y; lt[6 * i + 2] = Fa.z; lt[6 * i + 3] = Fl.x; lt[6 * i + 4] = Fl.y; lt[6 * i + 5] = Fl.z;
-        lt[18 + 3 * i] = h0; lt[19 + 3 * i] = h1; lt[20 + 3 * i] = h2;
-        lt[27 + i] = tau - Cb;
-        float* lk = linktab + (3 * k + i) * 8;
-        st4(lk, c1, s1, cy, sy); st4(lk + 4, po.x, po.y, po.z, 0.f);
+        lt[kLgF + 6 * i] = Fa.x; lt[kLgF + 6 * i + 1] = Fa.y; lt[kLgF + 6 * i + 2] = Fa.z;
+        lt[kLgF + 6 * i + 3] = Fl.x; lt[kLgF + 6 * i + 4] = Fl.y; lt[kLgF + 6 * i + 5] = Fl.z;
+        lt[kLgH + 3 * i] = h0; lt[kLgH + 3 * i + 1] = h1; lt[kLgH + 3 * i + 2] = h2;
+        lt[kLgRhs + i] = tau - Cb;
+        float* lk = linktab + (3 * k + i) * kLinkW;
+        st4(lk + kLkC1, c1, s1, cy, sy); st4(lk + kLkP, po.x, po.y, po.z, 0.f);
         if (i == 0) {
-          lt[30] = mc_; lt[31] = hc.x; lt[32] = hc.y; lt[33] = hc.z;
-          lt[34] = Ic.xx; lt[35] = Ic.xy; lt[36] = Ic.xz; lt[37] = Ic.yy; lt[38] = Ic.yz; lt[39] = Ic.zz;
-          lt[40] = f.a.x; lt[41] = f.a.y; lt[42] = f.a.z; lt[43] = f.l.x; lt[44] = f.l.y; lt[45] = f.l.z;
+          lt[kLgMass] = mc_; lt[kLgMom] = hc.x; lt[kLgMom + 1] = hc.y; lt[kLgMom + 2] = hc.z;
+          lt[kLgI] = Ic.xx; lt[kLgI + 1] = Ic.xy; lt[kLgI + 2] = Ic.xz; lt[kLgI + 3] = Ic.yy; lt[kLgI + 4] = Ic.yz; lt[kLgI + 5] = Ic.zz;
+          lt[kLgBias] = f.a.x; lt[kLgBias + 1] = f.a.y; lt[kLgBias + 2] = f.a.z; lt[kLgBias + 3] = f.l.x; lt[kLgBias + 4] = f.l.y; lt[kLgBias + 5] = f.l.z;
         }
       } else if (k == 0) {
-        envtab[0] = f.a.x; envtab[1] = f.a.y; envtab[2] = f.a.z; envtab[3] = f.l.x; envtab[4] = f.l.y; envtab[5] = f.l.z;
+        envtab[kEvBias] = f.a.x; envtab[kEvBias + 1] = f.a.y; envtab[kEvBias + 2] = f.a.z;
+        envtab[kEvBias + 3] = f.l.x; envtab[kEvBias + 4] = f.l.y; envtab[kEvBias + 5] = f.l.z;
       }
     }
     __syncwarp();
@@ -917,12 +972,12 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
     float W[3][6], L10, L20, L21, di[3], u[3];
     float m6[21], z0[6];
     {
-      const float* lt = legtab + k * 48;
+      const float* lt = legtab + k * kLegW;
 #pragma unroll
       for (int m = 0; m < 3; m++)
 #pragma unroll
-        for (int t = 0; t < 6; t++) W[m][t] = lt[6 * m + t];
-      const float H00 = lt[18], H10 = lt[21], H11 = lt[22], H20 = lt[24], H21 = lt[25], H22 = lt[26];
+        for (int t = 0; t < 6; t++) W[m][t] = lt[kLgF + 6 * m + t];
+      const float H00 = lt[kLgH], H10 = lt[kLgH + 3], H11 = lt[kLgH + 4], H20 = lt[kLgH + 6], H21 = lt[kLgH + 7], H22 = lt[kLgH + 8];
       di[0] = 1.0f / H00;
       L10 = H10 * di[0]; L20 = H20 * di[0];
       const float d1 = fmaf(-L10, H10, H11);
@@ -936,13 +991,13 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
         W[1][t] = fmaf(-L10, W[0][t], W[1][t]);
         W[2][t] = fmaf(-L20, W[0][t], fmaf(-L21, W[1][t], W[2][t]));
       }
-      u[0] = lt[27]; u[1] = fmaf(-L10, u[0], lt[28]); u[2] = fmaf(-L20, u[0], fmaf(-L21, u[1], lt[29]));
-      const float cm = lt[30];
-      const V3 ch_ = ld3(lt + 31);
+      u[0] = lt[kLgRhs]; u[1] = fmaf(-L10, u[0], lt[kLgRhs + 1]); u[2] = fmaf(-L20, u[0], fmaf(-L21, u[1], lt[kLgRhs + 2]));
+      const float cm = lt[kLgMass];
+      const V3 ch_ = ld3(lt + kLgMom);
       const M3 hx = skew(ch_);
       // packed lower triangle of [[A, B], [B^T, C]] : rows 0-2 = A, rows 3-5 = [B^T, C]
-      m6[tri(0, 0)] = lt[34]; m6[tri(1, 0)] = lt[35]; m6[tri(1, 1)] = lt[37];
-      m6[tri(2, 0)] = lt[36]; m6[tri(2, 1)] = lt[38]; m6[tri(2, 2)] = lt[39];
+      m6[tri(0, 0)] = lt[kLgI]; m6[tri(1, 0)] = lt[kLgI + 1]; m6[tri(1, 1)] = lt[kLgI + 3];         // xx xy xz yy yz zz
+      m6[tri(2, 0)] = lt[kLgI + 2]; m6[tri(2, 1)] = lt[kLgI + 4]; m6[tri(2, 2)] = lt[kLgI + 5];
       m6[tri(3, 0)] = hx.a00; m6[tri(3, 1)] = hx.a10; m6[tri(3, 2)] = hx.a20;
       m6[tri(4, 0)] = hx.a01; m6[tri(4, 1)] = hx.a11; m6[tri(4, 2)] = hx.a21;
       m6[tri(5, 0)] = hx.a02; m6[tri(5, 1)] = hx.a12; m6[tri(5, 2)] = hx.a22;
@@ -957,7 +1012,7 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
           for (int c = 0; c <= r; c++) m6[tri(r, c)] = fmaf(-wd, W[m][c], m6[tri(r, c)]);
         }
 #pragma unroll
-        for (int t = 0; t < 6; t++) z0[t] = (m == 0 ? lt[40 + t] : z0[t]) + ud * W[m][t];
+        for (int t = 0; t < 6; t++) z0[t] = (m == 0 ? lt[kLgBias + t] : z0[t]) + ud * W[m][t];
       }
       // the four legs (xor 1, 2 stay inside the group of lanes with the same link index)
 #pragma unroll
@@ -973,7 +1028,7 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
       m6[tri(5, 0)] += bx.a02; m6[tri(5, 1)] += bx.a12; m6[tri(5, 2)] += bx.a22;
       m6[tri(3, 3)] += bm; m6[tri(4, 4)] += bm; m6[tri(5, 5)] += bm;
 #pragma unroll
-      for (int t = 0; t < 6; t++) z0[t] += envtab[t];
+      for (int t = 0; t < 6; t++) z0[t] += envtab[kEvBias + t];
     }
     float a0[6];
     {
@@ -984,7 +1039,7 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
       chol6_solve(ch, bneg, a0);                // acceleration relative to free fall (gravity as a fictitious base acceleration)
       if (l16 == 0) {                           // the factor is needed again by the row images and the final back substitution
 #pragma unroll
-        for (int t = 0; t < 21; t++) envtab[8 + t] = ch.l[t];
+        for (int t = 0; t < 21; t++) envtab[kEvChol + t] = ch.l[t];
       }
     }
     // ---------------- joint accelerations of this lane's leg, velocity prediction v* = clamp(v + a dt)
@@ -1006,17 +1061,18 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
     wbs = tmul(R, ww); vbs = tmul(R, vw);
     __syncwarp();                                     // every lane has read F / H: the leg table becomes the rows' table
     if (l16 == 0) {                                   // predicted base velocity for the rows' right-hand sides (any lane of the warp may build them)
-      envtab[0] = wbs.x; envtab[1] = wbs.y; envtab[2] = wbs.z; envtab[3] = vbs.x; envtab[4] = vbs.y; envtab[5] = vbs.z;
+      envtab[kEvVel] = wbs.x; envtab[kEvVel + 1] = wbs.y; envtab[kEvVel + 2] = wbs.z;
+      envtab[kEvVel + 3] = vbs.x; envtab[kEvVel + 4] = vbs.y; envtab[kEvVel + 5] = vbs.z;
     }
     if (i == 0) {
-      float* lt = legtab + k * 48;
+      float* lt = legtab + k * kLegW;
 #pragma unroll
       for (int m = 0; m < 3; m++)
 #pragma unroll
-        for (int t = 0; t < 6; t++) lt[6 * m + t] = W[m][t];
-      lt[18] = L10; lt[19] = L20; lt[20] = L21; lt[21] = di[0]; lt[22] = di[1]; lt[23] = di[2];
-      lt[24] = qd[0]; lt[25] = qd[1]; lt[26] = qd[2];
-      lt[28] = c3; lt[29] = s3;                       // for the fp64 clearance of the shank's spheres
+        for (int t = 0; t < 6; t++) lt[kLgW + 6 * m + t] = W[m][t];
+      lt[kLgL10] = L10; lt[kLgL20] = L20; lt[kLgL21] = L21; lt[kLgDinv] = di[0]; lt[kLgDinv + 1] = di[1]; lt[kLgDinv + 2] = di[2];
+      lt[kLgQd] = qd[0]; lt[kLgQd + 1] = qd[1]; lt[kLgQd + 2] = qd[2];
+      lt[kLgC3] = c3; lt[kLgS3] = s3;
     }
     }   // ================ end of the forward dynamics
     T16_MARK(1);
@@ -1026,18 +1082,16 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
     if (ENV == 0 && P.has_ob && sub == P.substeps - 1) {
       const int o0 = mc.ob_off[clip], n_ob = mc.ob_off[clip + 1] - o0;
       if (n_ob > 0) {
-        const float* lk = linktab + 24 * k;
-        const float c1 = lk[0], s1 = lk[1], c2 = lk[10], s2 = lk[11], c23 = lk[18], s23 = lk[19];
-        const V3 p1 = ld3(lk + 4), p2 = ld3(lk + 12), p3 = ld3(lk + 20);
-        const V3 fb = p3 + rot<0>(rot<1>(ld3(L.foot), c23, s23), c1, s1);     // foot centre of this lane's leg
+        const LegFrames lf = leg_frames(linktab, k);
+        const V3 fb = lf.on_shank(ld3(L.foot));                                      // foot centre of this lane's leg
         const double* ob = mc.ob_table + (size_t)(o0 + ob_id) * 4;
         float sy_, cy_;
         llq_sincosf((float)ob[3], &sy_, &cy_);
         const V3 org = V3{(float)(px - ob[1]), (float)(py - ob[2]), (float)pz};      // base position relative to the plate centre
-        const V3 wh = p2 + rot<0>(rot<1>(ld3(M.wheel_off[k]), c2, s2), c1, s1);
+        const V3 wh = lf.on_thigh(ld3(M.wheel_off[k]));
         bool hit = plate_hit(org + mul(R, fb), L.foot_r, cy_, sy_, P.ob_hx, P.ob_hy, P.ob_hz, P.breaking);
         hit = hit || plate_hit(org + mul(R, wh), M.wheel_r[k], cy_, sy_, P.ob_hx, P.ob_hy, P.ob_hz, P.breaking);
-        hit = hit || plate_hit(org + mul(R, p1), M.hip_r[k], cy_, sy_, P.ob_hx, P.ob_hy, P.ob_hz, P.breaking);
+        hit = hit || plate_hit(org + mul(R, lf.p1), M.hip_r[k], cy_, sy_, P.ob_hx, P.ob_hy, P.ob_hz, P.breaking);
         hit = hit || plate_hit(org + mul(R, ld3(M.corner[2 * k])), 0.f, cy_, sy_, P.ob_hx, P.ob_hy, P.ob_hz, P.breaking);
         hit = hit || plate_hit(org + mul(R, ld3(M.corner[2 * k + 1])), 0.f, cy_, sy_, P.ob_hx, P.ob_hy, P.ob_hz, P.breaking);
         ob_hit = hit;
@@ -1048,12 +1102,10 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
       float* srow = s_new[el];
       const float* prow = s_new[el ^ 1];
       const V3 pw = V3{(float)px, (float)py, (float)pz};
-      const float* lk = linktab + 24 * k;
-      const float c1 = lk[0], s1 = lk[1], c2 = lk[10], s2 = lk[11], c23 = lk[18], s23 = lk[19];
-      const V3 p1 = ld3(lk + 4), p2 = ld3(lk + 12), p3 = ld3(lk + 20);
-      const V3 fb = p3 + rot<0>(rot<1>(ld3(L.foot), c23, s23), c1, s1);       // foot centre of this lane's leg
-      const V3 wh = pw + mul(R, p2 + rot<0>(rot<1>(ld3(M.wheel_off[k]), c2, s2), c1, s1));
-      const V3 hp_ = pw + mul(R, p1), ft = pw + mul(R, fb);
+      const LegFrames lf = leg_frames(linktab, k);
+      const V3 fb = lf.on_shank(ld3(L.foot));                                  // foot centre of this lane's leg
+      const V3 wh = pw + mul(R, lf.on_thigh(ld3(M.wheel_off[k])));
+      const V3 hp_ = pw + mul(R, lf.p1), ft = pw + mul(R, fb);
       const V3 c0 = pw + mul(R, ld3(M.corner[2 * k])), c1_ = pw + mul(R, ld3(M.corner[2 * k + 1]));
       if (i == 0) {
         float* o = srow + kSContactRec * k;
@@ -1102,8 +1154,8 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
         float lc1 = 1.f, ls1 = 0.f, lcy = 1.f, lsy = 0.f;
         V3 lp = V3{0.f, 0.f, 0.f};
         if (sdep > 0) {
-          const float* lk = linktab + (3 * sleg + sdep - 1) * 8;
-          const float4 a = ld4(lk), b4 = ld4(lk + 4);
+          const float* lk = linktab + (3 * sleg + sdep - 1) * kLinkW;
+          const float4 a = ld4(lk + kLkC1), b4 = ld4(lk + kLkP);
           lc1 = a.x; ls1 = a.y; lcy = a.z; lsy = a.w; lp = V3{b4.x, b4.y, b4.z};
         }
         const V3 cl = ld3(sp.c);
@@ -1136,12 +1188,12 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
             if (sdep > 0) {
               const LegConst& SL = M.leg[sleg];
               if (sdep == 3) {
-                const double dc3 = (double)legtab[sleg * 48 + 28], ds3 = (double)legtab[sleg * 48 + 29];
+                const double dc3 = (double)legtab[sleg * kLegW + kLgC3], ds3 = (double)legtab[sleg * kLegW + kLgS3];
                 t = dc3 * x + ds3 * z; z = -ds3 * x + dc3 * z; x = t;            // Ry(theta3)
                 x += (double)SL.j[2].r[0]; y += (double)SL.j[2].r[1]; z += (double)SL.j[2].r[2];
               }
               if (sdep >= 2) {
-                const double dc2 = (double)linktab[(3 * sleg + 1) * 8 + 2], ds2 = (double)linktab[(3 * sleg + 1) * 8 + 3];
+                const double dc2 = (double)linktab[(3 * sleg + 1) * kLinkW + kLkCy], ds2 = (double)linktab[(3 * sleg + 1) * kLinkW + kLkSy];
                 t = dc2 * x + ds2 * z; z = -ds2 * x + dc2 * z; x = t;            // Ry(theta2)
                 x += (double)SL.j[1].r[0]; y += (double)SL.j[1].r[1]; z += (double)SL.j[1].r[2];
               }
@@ -1226,11 +1278,11 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
           }
           const V3 Pc = cb - sp.r * dn;                   // contact point on the sphere surface
           float* cr = contab + idx * kConW;
-          st4(cr, __int_as_float(sdep > 0 ? sleg : -1), __int_as_float(sdep), Pc.x, Pc.y);
-          st4(cr + 4, Pc.z, dn.x, dn.y, dn.z);
-          st4(cr + 8, d1_.x, d1_.y, d1_.z, d2_.x);
-          st4(cr + 12, d2_.y, d2_.z, dist, sp.foot ? mu_foot : sp.mu_link);
-          cr[16] = P.warm * warm[rd]; cr[17] = 0.f;
+          st4(cr + kCoLeg, __int_as_float(sdep > 0 ? sleg : -1), __int_as_float(sdep), Pc.x, Pc.y);
+          st4(cr + (kCoPc + 2), Pc.z, dn.x, dn.y, dn.z);
+          st4(cr + (kCoDir + 3), d1_.x, d1_.y, d1_.z, d2_.x);
+          st4(cr + (kCoDir + 7), d2_.y, d2_.z, dist, sp.foot ? mu_foot : sp.mu_link);
+          cr[kCoLam0] = P.warm * warm[rd]; cr[kCoLam] = 0.f;
           mycon[rd] = idx;
         } else {
           warm[rd] = 0.f;                                 // manifold point removed: no warm start
@@ -1252,7 +1304,7 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
       nl = __popc(bal);
       const int rk = __popc(bal & lowmask);
       if (dir != 0.f) {
-        if (rk < kMaxLim) st4(limtab + rk * 4, __int_as_float(k), __int_as_float(i), dir, pen);
+        if (rk < kMaxLim) st4(limtab + rk * kLimW + kLmLeg, __int_as_float(k), __int_as_float(i), dir, pen);
         else n_overflow += 1;
       }
       if (nl > kMaxLim) nl = kMaxLim;
@@ -1307,7 +1359,7 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
           in.Cmax = two_pass ? (pass == 0 ? cA : cB) : max(cA, cB);
           in.Lmax = two_pass ? (pass == 0 ? lA : lB) : max(lA, lB);
           const bool upper = lane >= 16;
-          in.res = (two_pass && upper != (pass == 1)) ? nullptr : (upper ? tbB : tbA) + (kLinkTab + kLegTab + kConTab + kLimTab);
+          in.res = (two_pass && upper != (pass == 1)) ? nullptr : (upper ? tbB : tbA) + (kRowOff + kResBase);
           solve_rows(in);
           __syncwarp();
         }
@@ -1319,20 +1371,20 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
     if (nc | nl) {
       if (l16 == 0) { n_contact_rows += 3u * (unsigned)nc; n_limit_rows += (unsigned)nl; }
 #pragma unroll
-      for (int rd = 0; rd < 2; rd++) if (mycon[rd] >= 0) warm[rd] = contab[mycon[rd] * kConW + 17];
+      for (int rd = 0; rd < 2; rd++) if (mycon[rd] >= 0) warm[rd] = contab[mycon[rd] * kConW + kCoLam];
       // ---- total impulse -> velocity change: one back substitution for the base, one 3x3 solve per leg
-      const float4 y0 = ld4(rowtab), y1 = ld4(rowtab + 4);
+      const float4 y0 = ld4(rowtab + kResBase), y1 = ld4(rowtab + (kResBase + 4));
       const float Yt[6] = {y0.x, y0.y, y0.z, y0.w, y1.x, y1.y};
-      const float om[3] = {rowtab[6 + 3 * k], rowtab[7 + 3 * k], rowtab[8 + 3 * k]};
-      chol6_bwd_p(envtab + 8, Yt, dvb);
-      const float* lt = legtab + k * 48;            // W, L, D^-1 of this lane's leg come back from the leg table (not kept live across the solve)
+      const float om[3] = {rowtab[kResLeg + 3 * k], rowtab[kResLeg + 1 + 3 * k], rowtab[kResLeg + 2 + 3 * k]};
+      chol6_bwd_p(envtab + kEvChol, Yt, dvb);
+      const float* lt = legtab + k * kLegW;        // W, L, D^-1 of this lane's leg come back from the leg table (not kept live across the solve)
       float t3[3];
 #pragma unroll
       for (int m = 0; m < 3; m++) {
-        const float wm[6] = {lt[6 * m], lt[6 * m + 1], lt[6 * m + 2], lt[6 * m + 3], lt[6 * m + 4], lt[6 * m + 5]};
-        t3[m] = (om[m] - dot6(wm, dvb)) * lt[21 + m];
+        const float wm[6] = {lt[kLgW + 6 * m], lt[kLgW + 6 * m + 1], lt[kLgW + 6 * m + 2], lt[kLgW + 6 * m + 3], lt[kLgW + 6 * m + 4], lt[kLgW + 6 * m + 5]};
+        t3[m] = (om[m] - dot6(wm, dvb)) * lt[kLgDinv + m];
       }
-      dvl[2] = t3[2]; dvl[1] = fmaf(-lt[20], dvl[2], t3[1]); dvl[0] = fmaf(-lt[18], dvl[1], fmaf(-lt[19], dvl[2], t3[0]));
+      dvl[2] = t3[2]; dvl[1] = fmaf(-lt[kLgL21], dvl[2], t3[1]); dvl[0] = fmaf(-lt[kLgL10], dvl[1], fmaf(-lt[kLgL20], dvl[2], t3[0]));
     }
     __syncwarp();              // the row table is the next sub-step's scratch
     T16_MARK(3);
@@ -1419,8 +1471,8 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
     const int tsrc = tel < EPB ? tel : EPB - 1;
     const int tenv_raw = blockIdx.x * EPB + tsrc;
     const float* tbase = s_env_dyn + tsrc * kEnvFloats;
-    step_tail<ENV>(E, mc, P, M, s_new[0], s_hist[0], *reinterpret_cast<const TailState*>(tbase + (rowtab - linktab)),
-                        tbase + (envtab - linktab) + 44, obs2, obs2_ld, winner, seed, gid0, record, tel, tk, tenv_raw < N ? tenv_raw : N - 1, tval);
+    step_tail<ENV>(E, mc, P, M, s_new[0], s_hist[0], *reinterpret_cast<const TailState*>(tbase + kRowOff),
+                   tbase + (kEnvOff + kEvAct), obs2, obs2_ld, winner, seed, gid0, record, tel, tk, tenv_raw < N ? tenv_raw : N - 1, tval);
   }
   // ---- observation rows (history shift + new prop / action / future; EPMC / SEPMC: the 778 perception rays are cast while the row is
   // written): every warp of the CTA emits the rows of its own two envs, coalesced
