@@ -4,6 +4,9 @@
 //   * link lane   leg k = l & 3, link i = l >> 2 (0 hip, 1 thigh, 2 shank; i = 3: the base body): rigid-body inertia and bias
 //                 wrench of ONE body in base coordinates -> composite inertias (suffix sums along the leg) -> its column F_i of the
 //                 base/joint coupling block and its row of the leg's 3x3 joint-space inertia H_k (composite-rigid-body form);
+//   * factor lane on the first half of the CTA's warps only, 8 lanes per robot and four robots per warp (factorise_robot): the leg
+//                 factorisations, the base block's Cholesky factor and the velocity prediction, which are the same for every lane
+//                 of a leg or a robot and so cost a warp instruction per robot served; the other warps go on to the collision screen;
 //   * sphere lane collision spheres l and l + 16 of the robot (feet, knee wheels, hips, thighs, shanks, trunk corners) against
 //                 the ground / arena walls / corridor boxes, compacted into the env's contact list with one ballot;
 //   * row lane    ONE constraint row of the sub-step's LCP: its image (y, w) under the block factorisation of the mass matrix, its row
@@ -12,7 +15,7 @@
 //                 every sub-step (heaviest with lightest) and the rows of a pair are packed into the warp's 32 lanes -- a lane's row
 //                 may belong to either env of the pair, or (after the re-pairing) to an env another warp owns (see solve_rows).
 // The dynamics are the same equations Bullet's articulated-body algorithm solves, factorised block-wise instead of link by link:
-//   [ Ic  F ] [a0]   [-p0   ]        H_k = L D L^T per leg,  S = Ic - sum_k F_k H_k^-1 F_k^T = L0 L0^T  (6x6, replicated),
+//   [ Ic  F ] [a0]   [-p0   ]        H_k = L D L^T per leg,  S = Ic - sum_k F_k H_k^-1 F_k^T = L0 L0^T  (6x6, per robot),
 //   [ F^T H ] [qdd] = [tau - C]       J M^-1 J'^T = y.y' + [same leg] w.(D^-1 w'),  y = L0^-1 (G - F_k H_k^-1 j),  w = L^-1 j.
 // Everything is expressed in base coordinates about the base reference point (an inertial frame that coincides with the base at
 // the start of the sub-step), so composite inertias and bias wrenches simply add.
@@ -41,6 +44,7 @@ struct alignas(16) SphTable { int n; int rule; int pad[2]; SphConst s[kMaxSph]; 
 // link record 3 k + i (body i of leg k): rotation Rx(c1, s1) Ry(cy, sy) and origin p of the body, base coordinates
 constexpr int kLinkW = 8, kLinkTab = 12 * kLinkW;
 constexpr int kLkC1 = 0, kLkS1 = 1, kLkCy = 2, kLkSy = 3, kLkP = 4;
+constexpr int kLkQd = 7;                                 // dynamics phase: velocity of the body's joint at the start of the sub-step
 // leg record k, dynamics phase: the leg's blocks of the mass matrix and what its composite rigid body carries
 constexpr int kLegW = 48, kLegTab = 4 * kLegW;
 constexpr int kLgF = 0;                                  // coupling block F_k: one 6-vector per joint
@@ -48,11 +52,11 @@ constexpr int kLgH = 18;                                 // joint-space inertia 
 constexpr int kLgRhs = 27;                               // tau - C per joint (3)
 constexpr int kLgMass = 30, kLgMom = 31, kLgI = 34;      // the leg as one body: mass, first moment (3), inertia (Sym3 order, 6)
 constexpr int kLgBias = 40;                              // accumulated bias wrench of the leg (6)
-// leg record k, rows phase (from the __syncwarp that ends the dynamics): the factorised leg and its predicted joint velocities
+constexpr int kLgC3 = 46, kLgS3 = 47;                    // both phases: knee cosine and sine (fp64 centres of the shank's spheres)
+// leg record k, rows phase (from the __syncwarp in factorise_robot): the factorised leg and its predicted joint velocities
 constexpr int kLgW = 0;                                  // W = F L^-T: one 6-vector per joint
 constexpr int kLgL10 = 18, kLgL20 = 19, kLgL21 = 20;     // H_k = L D L^T
 constexpr int kLgDinv = 21, kLgQd = 24;                  // D^-1 (3), predicted joint velocities (3)
-constexpr int kLgC3 = 28, kLgS3 = 29;                    // knee cosine and sine (fp64 centres of the shank's spheres)
 // contact record, one per manifold point
 constexpr int kConW = 20, kConTab = kMaxCon * kConW;
 constexpr int kCoLeg = 0, kCoDepth = 1;                  // leg of the sphere's link (-1: the base), depth of the link (int bits)
@@ -73,11 +77,14 @@ constexpr int kScBias = 0, kScMass = 6, kScMom = 7, kScI = 10;   // bias wrench 
 // ... the totals of the env's rows after the sweep (18 floats at its head), and after the last sub-step the TailState
 constexpr int kResBase = 0, kResLeg = 6;                 // sum lam y (6); per leg k, sum lam w at kResLeg + 3 k
 // env record (one per env)
-constexpr int kEnvTab = 56;
+constexpr int kEnvTab = 72;
 constexpr int kEvBias = 0;                               // dynamics phase: bias wrench of the base body (6)
 constexpr int kEvVel = 0;                                // rows phase: predicted base velocity w, v (base coordinates, 6)
 constexpr int kEvChol = 8;                               // Cholesky factor of the base block (21, packed as in llq_math.cuh)
 constexpr int kEvTarget = 32, kEvAct = 44;               // clipped joint targets (12), actions (12)
+constexpr int kEvQp = 56;                                // dynamics phase: base orientation (URDF body axes, 4)
+constexpr int kEvW0 = 60;                                // dynamics phase: base velocity w, v at the start of the sub-step (world, 6)
+constexpr int kEvWp = 66;                                // rows phase: predicted base velocity w, v (world, 6)
 constexpr int kATabWarp = 32 * 32;     // Delassus coefficients of one WARP (its two envs' rows packed into 32 lanes): atab[col * 32 + lane]
 constexpr int kEnvFloats = 944;        // >= the sum of the tables, and = 16 (mod 32): envs an odd number of slots apart hit disjoint banks
 static_assert(16 * kScrW <= kRowTab && kResLeg + 4 * 3 <= kRowTab, "the row table's other uses fit in it");
@@ -181,6 +188,133 @@ LLQ_DI void sphere_box(double wx, double wy, double wz, double r, const float* b
     if (h2 - p2 < best) { best = h2 - p2; nn = V3{0.f, 0.f, 1.f}; }
     if (h2 + p2 < best) { best = h2 + p2; nn = V3{0.f, 0.f, -1.f}; }
     db = -best - r;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Second half of the forward dynamics: the per-robot factorisation of the mass matrix and the velocity prediction, on 8 lanes per
+// robot (lane l8: leg k = l8 & 3, each leg replicated on 2 lanes, the base block on all 8) so that one warp serves four robots.  It
+// starts from what the robot's 16 link lanes left in its tables (leg blocks F, H, rhs and composite body, the base body's bias wrench,
+// the state at the start of the sub-step) and leaves the rows-phase tables: leg factors W, L, D^-1, predicted joint velocities, the
+// base block's Cholesky factor, the predicted base velocity in base and in world coordinates.  The arithmetic and its order are
+// those of a 16-lane robot: the sums over the legs are the same two xor shuffles.
+LLQ_DI void factorise_robot(float* tb, int k, bool lead, bool legw, const ModelConst& M, const StepParams& P) {
+  float* const legtab = tb + kLegOff;
+  float* const envtab = tb + kEnvOff;
+  const float dt = P.dt;
+  const Q4 qp = Q4{envtab[kEvQp], envtab[kEvQp + 1], envtab[kEvQp + 2], envtab[kEvQp + 3]};
+  V3 ww = ld3(envtab + kEvW0), vw = ld3(envtab + (kEvW0 + 3));
+  float qd[3];
+#pragma unroll
+  for (int t = 0; t < 3; t++) qd[t] = tb[kLinkOff + (3 * k + t) * kLinkW + kLkQd];
+  const M3 R = qmat(qp);                       // world <- B'
+  const V3 wb = tmul(R, ww), vb = tmul(R, vw);     // base velocity, base coordinates
+  // ---------------- per leg (replicated on its 2 lanes): H_k = L D L^T, Schur complement and right-hand side of the base
+  float W[3][6], L10, L20, L21, di[3], u[3];
+  float m6[21], z0[6];
+  {
+    const float* lt = legtab + k * kLegW;
+#pragma unroll
+    for (int m = 0; m < 3; m++)
+#pragma unroll
+      for (int t = 0; t < 6; t++) W[m][t] = lt[kLgF + 6 * m + t];
+    const float H00 = lt[kLgH], H10 = lt[kLgH + 3], H11 = lt[kLgH + 4], H20 = lt[kLgH + 6], H21 = lt[kLgH + 7], H22 = lt[kLgH + 8];
+    di[0] = 1.0f / H00;
+    L10 = H10 * di[0]; L20 = H20 * di[0];
+    const float d1 = fmaf(-L10, H10, H11);
+    di[1] = 1.0f / d1;
+    L21 = fmaf(-L20, H10, H21) * di[1];
+    const float d2 = fmaf(-L20, H20, fmaf(-L21 * L21, d1, H22));
+    di[2] = 1.0f / d2;
+    // W = F L^-T (columns w_m), u = L^-1 rhs
+#pragma unroll
+    for (int t = 0; t < 6; t++) {
+      W[1][t] = fmaf(-L10, W[0][t], W[1][t]);
+      W[2][t] = fmaf(-L20, W[0][t], fmaf(-L21, W[1][t], W[2][t]));
+    }
+    u[0] = lt[kLgRhs]; u[1] = fmaf(-L10, u[0], lt[kLgRhs + 1]); u[2] = fmaf(-L20, u[0], fmaf(-L21, u[1], lt[kLgRhs + 2]));
+    const float cm = lt[kLgMass];
+    const V3 ch_ = ld3(lt + kLgMom);
+    const M3 hx = skew(ch_);
+    // packed lower triangle of [[A, B], [B^T, C]] : rows 0-2 = A, rows 3-5 = [B^T, C]
+    m6[tri(0, 0)] = lt[kLgI]; m6[tri(1, 0)] = lt[kLgI + 1]; m6[tri(1, 1)] = lt[kLgI + 3];         // xx xy xz yy yz zz
+    m6[tri(2, 0)] = lt[kLgI + 2]; m6[tri(2, 1)] = lt[kLgI + 4]; m6[tri(2, 2)] = lt[kLgI + 5];
+    m6[tri(3, 0)] = hx.a00; m6[tri(3, 1)] = hx.a10; m6[tri(3, 2)] = hx.a20;
+    m6[tri(4, 0)] = hx.a01; m6[tri(4, 1)] = hx.a11; m6[tri(4, 2)] = hx.a21;
+    m6[tri(5, 0)] = hx.a02; m6[tri(5, 1)] = hx.a12; m6[tri(5, 2)] = hx.a22;
+    m6[tri(3, 3)] = cm; m6[tri(4, 3)] = 0.f; m6[tri(4, 4)] = cm; m6[tri(5, 3)] = 0.f; m6[tri(5, 4)] = 0.f; m6[tri(5, 5)] = cm;
+#pragma unroll
+    for (int m = 0; m < 3; m++) {
+      const float ud = u[m] * di[m];
+#pragma unroll
+      for (int r = 0; r < 6; r++) {
+        const float wd = W[m][r] * di[m];
+#pragma unroll
+        for (int c = 0; c <= r; c++) m6[tri(r, c)] = fmaf(-wd, W[m][c], m6[tri(r, c)]);
+      }
+#pragma unroll
+      for (int t = 0; t < 6; t++) z0[t] = (m == 0 ? lt[kLgBias + t] : z0[t]) + ud * W[m][t];
+    }
+    // the four legs (xor 1, 2 stay inside the robot's group of four lanes)
+#pragma unroll
+    for (int t = 0; t < 21; t++) m6[t] = gsum4(m6[t]);
+#pragma unroll
+    for (int t = 0; t < 6; t++) z0[t] = gsum4(z0[t]);
+    const V3 bh = ld3(M.base.h); const Sym3 bI = ldsym(M.base.I); const float bm = M.base.m;
+    const M3 bx = skew(bh);
+    m6[tri(0, 0)] += bI.xx; m6[tri(1, 0)] += bI.xy; m6[tri(1, 1)] += bI.yy;
+    m6[tri(2, 0)] += bI.xz; m6[tri(2, 1)] += bI.yz; m6[tri(2, 2)] += bI.zz;
+    m6[tri(3, 0)] += bx.a00; m6[tri(3, 1)] += bx.a10; m6[tri(3, 2)] += bx.a20;
+    m6[tri(4, 0)] += bx.a01; m6[tri(4, 1)] += bx.a11; m6[tri(4, 2)] += bx.a21;
+    m6[tri(5, 0)] += bx.a02; m6[tri(5, 1)] += bx.a12; m6[tri(5, 2)] += bx.a22;
+    m6[tri(3, 3)] += bm; m6[tri(4, 4)] += bm; m6[tri(5, 5)] += bm;
+#pragma unroll
+    for (int t = 0; t < 6; t++) z0[t] += envtab[kEvBias + t];
+  }
+  float a0[6];
+  {
+    const Chol6 ch = chol6(m6);
+    float bneg[6];
+#pragma unroll
+    for (int t = 0; t < 6; t++) bneg[t] = -z0[t];
+    chol6_solve(ch, bneg, a0);                // acceleration relative to free fall (gravity as a fictitious base acceleration)
+    if (lead) {                               // the factor is needed again by the row images and the final back substitution
+#pragma unroll
+      for (int t = 0; t < 21; t++) envtab[kEvChol + t] = ch.l[t];
+    }
+  }
+  // ---------------- joint accelerations of this lane's leg, velocity prediction v* = clamp(v + a dt)
+  {
+    float t3[3];
+#pragma unroll
+    for (int m = 0; m < 3; m++) t3[m] = (u[m] - dot6(W[m], a0)) * di[m];
+    // qdd = L^-T t3
+    const float a2 = t3[2], a1 = fmaf(-L21, a2, t3[1]), a0j = fmaf(-L10, a1, fmaf(-L20, a2, t3[0]));
+    const float qdd[3] = {a0j, a1, a2};
+    const V3 wd = mul(R, V3{a0[0], a0[1], a0[2]});
+    V3 vd = mul(R, V3{a0[3], a0[4], a0[5]} + cross(wb, vb));
+    vd.z += P.gz;
+    ww = V3{clampf(fmaf(wd.x, dt, ww.x), -P.vmax, P.vmax), clampf(fmaf(wd.y, dt, ww.y), -P.vmax, P.vmax), clampf(fmaf(wd.z, dt, ww.z), -P.vmax, P.vmax)};
+    vw = V3{clampf(fmaf(vd.x, dt, vw.x), -P.vmax, P.vmax), clampf(fmaf(vd.y, dt, vw.y), -P.vmax, P.vmax), clampf(fmaf(vd.z, dt, vw.z), -P.vmax, P.vmax)};
+#pragma unroll
+    for (int t = 0; t < 3; t++) qd[t] = clampf(fmaf(qdd[t], dt, qd[t]), -P.vmax, P.vmax);
+  }
+  const V3 wbs = tmul(R, ww), vbs = tmul(R, vw);    // predicted base velocity in base coordinates (the rows' generalised velocity)
+  __syncwarp();                                     // every lane has read F / H / the base bias: they become the rows' tables
+  if (lead) {
+    envtab[kEvVel] = wbs.x; envtab[kEvVel + 1] = wbs.y; envtab[kEvVel + 2] = wbs.z;
+    envtab[kEvVel + 3] = vbs.x; envtab[kEvVel + 4] = vbs.y; envtab[kEvVel + 5] = vbs.z;
+    envtab[kEvWp] = ww.x; envtab[kEvWp + 1] = ww.y; envtab[kEvWp + 2] = ww.z;
+    envtab[kEvWp + 3] = vw.x; envtab[kEvWp + 4] = vw.y; envtab[kEvWp + 5] = vw.z;
+  }
+  if (legw) {
+    float* lt = legtab + k * kLegW;
+#pragma unroll
+    for (int m = 0; m < 3; m++)
+#pragma unroll
+      for (int t = 0; t < 6; t++) lt[kLgW + 6 * m + t] = W[m][t];
+    lt[kLgL10] = L10; lt[kLgL20] = L20; lt[kLgL21] = L21; lt[kLgDinv] = di[0]; lt[kLgDinv + 1] = di[1]; lt[kLgDinv + 2] = di[2];
+    lt[kLgQd] = qd[0]; lt[kLgQd + 1] = qd[1]; lt[kLgQd + 2] = qd[2];
   }
 }
 
@@ -725,7 +859,7 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
                                                             unsigned long long seed, long long gid0, int record) {
   constexpr int BLOCK = LLQ16_BLOCK, EPB = BLOCK / 16;        // 2 envs per warp
   constexpr int EPT = (EPB + 7) / 8 * 8;                      // the tail runs 8 envs per warp on whole warps: rows EPB.. are dummies
-  static_assert(BLOCK % 32 == 0 && EPB <= 32, "whole warps; one lane per env in the pairing");
+  static_assert(BLOCK % 64 == 0 && EPB <= 32, "an even number of warps (factor warps w and w + BLOCK / 64); one lane per env in the pairing");
   __shared__ __align__(16) ModelConst M;
   __shared__ __align__(16) SphTable ST;
   __shared__ __align__(16) float s_new[EPT][kNewObs];
@@ -863,7 +997,6 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
         push_on = push_count < P.push_duration;
       }
     }
-    V3 wbs, vbs;                                  // predicted base velocity in base coordinates (the rows' generalised velocity)
     {   // ================ forward dynamics; everything declared here dies at the closing brace (register budget of the solver)
     // ---------------- kinematics: every lane evaluates the sine / cosine of its own joint, the leg's six values go round by shuffle
     const M3 R = qmat(qp);                       // world <- B'
@@ -956,125 +1089,36 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
         lt[kLgH + 3 * i] = h0; lt[kLgH + 3 * i + 1] = h1; lt[kLgH + 3 * i + 2] = h2;
         lt[kLgRhs + i] = tau - Cb;
         float* lk = linktab + (3 * k + i) * kLinkW;
-        st4(lk + kLkC1, c1, s1, cy, sy); st4(lk + kLkP, po.x, po.y, po.z, 0.f);
+        st4(lk + kLkC1, c1, s1, cy, sy); st4(lk + kLkP, po.x, po.y, po.z, qdi);
         if (i == 0) {
           lt[kLgMass] = mc_; lt[kLgMom] = hc.x; lt[kLgMom + 1] = hc.y; lt[kLgMom + 2] = hc.z;
           lt[kLgI] = Ic.xx; lt[kLgI + 1] = Ic.xy; lt[kLgI + 2] = Ic.xz; lt[kLgI + 3] = Ic.yy; lt[kLgI + 4] = Ic.yz; lt[kLgI + 5] = Ic.zz;
           lt[kLgBias] = f.a.x; lt[kLgBias + 1] = f.a.y; lt[kLgBias + 2] = f.a.z; lt[kLgBias + 3] = f.l.x; lt[kLgBias + 4] = f.l.y; lt[kLgBias + 5] = f.l.z;
+          lt[kLgC3] = c3; lt[kLgS3] = s3;
         }
       } else if (k == 0) {
         envtab[kEvBias] = f.a.x; envtab[kEvBias + 1] = f.a.y; envtab[kEvBias + 2] = f.a.z;
         envtab[kEvBias + 3] = f.l.x; envtab[kEvBias + 4] = f.l.y; envtab[kEvBias + 5] = f.l.z;
+        st4(envtab + kEvQp, qp.x, qp.y, qp.z, qp.w);
+        envtab[kEvW0] = ww.x; envtab[kEvW0 + 1] = ww.y; envtab[kEvW0 + 2] = ww.z;
+        envtab[kEvW0 + 3] = vw.x; envtab[kEvW0 + 4] = vw.y; envtab[kEvW0 + 5] = vw.z;
       }
     }
-    __syncwarp();
-    // ---------------- per leg (replicated on its 4 lanes): H_k = L D L^T, Schur complement and right-hand side of the base
-    float W[3][6], L10, L20, L21, di[3], u[3];
-    float m6[21], z0[6];
+    }   // ================ end of the link lanes' part of the forward dynamics
+    // ---------------- factorisation and velocity prediction (factorise_robot), four robots per warp: warp w < NW / 2 takes the
+    // robots of warps w and w + NW / 2, whose tables it waits for at named barrier 1 + w; the other warps only arrive there and go on
+    // to the collision screen (which reads the link table and the knee angles only).  Their tables are complete at the CTA barrier.
     {
-      const float* lt = legtab + k * kLegW;
-#pragma unroll
-      for (int m = 0; m < 3; m++)
-#pragma unroll
-        for (int t = 0; t < 6; t++) W[m][t] = lt[kLgF + 6 * m + t];
-      const float H00 = lt[kLgH], H10 = lt[kLgH + 3], H11 = lt[kLgH + 4], H20 = lt[kLgH + 6], H21 = lt[kLgH + 7], H22 = lt[kLgH + 8];
-      di[0] = 1.0f / H00;
-      L10 = H10 * di[0]; L20 = H20 * di[0];
-      const float d1 = fmaf(-L10, H10, H11);
-      di[1] = 1.0f / d1;
-      L21 = fmaf(-L20, H10, H21) * di[1];
-      const float d2 = fmaf(-L20, H20, fmaf(-L21 * L21, d1, H22));
-      di[2] = 1.0f / d2;
-      // W = F L^-T (columns w_m), u = L^-1 rhs
-#pragma unroll
-      for (int t = 0; t < 6; t++) {
-        W[1][t] = fmaf(-L10, W[0][t], W[1][t]);
-        W[2][t] = fmaf(-L20, W[0][t], fmaf(-L21, W[1][t], W[2][t]));
-      }
-      u[0] = lt[kLgRhs]; u[1] = fmaf(-L10, u[0], lt[kLgRhs + 1]); u[2] = fmaf(-L20, u[0], fmaf(-L21, u[1], lt[kLgRhs + 2]));
-      const float cm = lt[kLgMass];
-      const V3 ch_ = ld3(lt + kLgMom);
-      const M3 hx = skew(ch_);
-      // packed lower triangle of [[A, B], [B^T, C]] : rows 0-2 = A, rows 3-5 = [B^T, C]
-      m6[tri(0, 0)] = lt[kLgI]; m6[tri(1, 0)] = lt[kLgI + 1]; m6[tri(1, 1)] = lt[kLgI + 3];         // xx xy xz yy yz zz
-      m6[tri(2, 0)] = lt[kLgI + 2]; m6[tri(2, 1)] = lt[kLgI + 4]; m6[tri(2, 2)] = lt[kLgI + 5];
-      m6[tri(3, 0)] = hx.a00; m6[tri(3, 1)] = hx.a10; m6[tri(3, 2)] = hx.a20;
-      m6[tri(4, 0)] = hx.a01; m6[tri(4, 1)] = hx.a11; m6[tri(4, 2)] = hx.a21;
-      m6[tri(5, 0)] = hx.a02; m6[tri(5, 1)] = hx.a12; m6[tri(5, 2)] = hx.a22;
-      m6[tri(3, 3)] = cm; m6[tri(4, 3)] = 0.f; m6[tri(4, 4)] = cm; m6[tri(5, 3)] = 0.f; m6[tri(5, 4)] = 0.f; m6[tri(5, 5)] = cm;
-#pragma unroll
-      for (int m = 0; m < 3; m++) {
-        const float ud = u[m] * di[m];
-#pragma unroll
-        for (int r = 0; r < 6; r++) {
-          const float wd = W[m][r] * di[m];
-#pragma unroll
-          for (int c = 0; c <= r; c++) m6[tri(r, c)] = fmaf(-wd, W[m][c], m6[tri(r, c)]);
-        }
-#pragma unroll
-        for (int t = 0; t < 6; t++) z0[t] = (m == 0 ? lt[kLgBias + t] : z0[t]) + ud * W[m][t];
-      }
-      // the four legs (xor 1, 2 stay inside the group of lanes with the same link index)
-#pragma unroll
-      for (int t = 0; t < 21; t++) m6[t] = gsum4(m6[t]);
-#pragma unroll
-      for (int t = 0; t < 6; t++) z0[t] = gsum4(z0[t]);
-      const V3 bh = ld3(M.base.h); const Sym3 bI = ldsym(M.base.I); const float bm = M.base.m;
-      const M3 bx = skew(bh);
-      m6[tri(0, 0)] += bI.xx; m6[tri(1, 0)] += bI.xy; m6[tri(1, 1)] += bI.yy;
-      m6[tri(2, 0)] += bI.xz; m6[tri(2, 1)] += bI.yz; m6[tri(2, 2)] += bI.zz;
-      m6[tri(3, 0)] += bx.a00; m6[tri(3, 1)] += bx.a10; m6[tri(3, 2)] += bx.a20;
-      m6[tri(4, 0)] += bx.a01; m6[tri(4, 1)] += bx.a11; m6[tri(4, 2)] += bx.a21;
-      m6[tri(5, 0)] += bx.a02; m6[tri(5, 1)] += bx.a12; m6[tri(5, 2)] += bx.a22;
-      m6[tri(3, 3)] += bm; m6[tri(4, 4)] += bm; m6[tri(5, 5)] += bm;
-#pragma unroll
-      for (int t = 0; t < 6; t++) z0[t] += envtab[kEvBias + t];
-    }
-    float a0[6];
-    {
-      const Chol6 ch = chol6(m6);
-      float bneg[6];
-#pragma unroll
-      for (int t = 0; t < 6; t++) bneg[t] = -z0[t];
-      chol6_solve(ch, bneg, a0);                // acceleration relative to free fall (gravity as a fictitious base acceleration)
-      if (l16 == 0) {                           // the factor is needed again by the row images and the final back substitution
-#pragma unroll
-        for (int t = 0; t < 21; t++) envtab[kEvChol + t] = ch.l[t];
+      constexpr int NW2 = BLOCK / 64;
+      const int wq = tid >> 5;
+      if (wq < NW2) {
+        asm volatile("bar.sync %0, 64;" ::"r"(1 + wq) : "memory");
+        const int lane = tid & 31, q4 = lane >> 3;
+        factorise_robot(s_env_dyn + (2 * (wq + (q4 >> 1) * NW2) + (q4 & 1)) * kEnvFloats, lane & 3, (lane & 7) == 0, (lane & 7) < 4, M, P);
+      } else {
+        asm volatile("bar.arrive %0, 64;" ::"r"(1 + wq - NW2) : "memory");
       }
     }
-    // ---------------- joint accelerations of this lane's leg, velocity prediction v* = clamp(v + a dt)
-    {
-      float t3[3];
-#pragma unroll
-      for (int m = 0; m < 3; m++) t3[m] = (u[m] - dot6(W[m], a0)) * di[m];
-      // qdd = L^-T t3
-      const float a2 = t3[2], a1 = fmaf(-L21, a2, t3[1]), a0j = fmaf(-L10, a1, fmaf(-L20, a2, t3[0]));
-      const float qdd[3] = {a0j, a1, a2};
-      const V3 wd = mul(R, V3{a0[0], a0[1], a0[2]});
-      V3 vd = mul(R, V3{a0[3], a0[4], a0[5]} + cross(wb, vb));
-      vd.z += P.gz;
-      ww = V3{clampf(fmaf(wd.x, dt, ww.x), -P.vmax, P.vmax), clampf(fmaf(wd.y, dt, ww.y), -P.vmax, P.vmax), clampf(fmaf(wd.z, dt, ww.z), -P.vmax, P.vmax)};
-      vw = V3{clampf(fmaf(vd.x, dt, vw.x), -P.vmax, P.vmax), clampf(fmaf(vd.y, dt, vw.y), -P.vmax, P.vmax), clampf(fmaf(vd.z, dt, vw.z), -P.vmax, P.vmax)};
-#pragma unroll
-      for (int t = 0; t < 3; t++) qd[t] = clampf(fmaf(qdd[t], dt, qd[t]), -P.vmax, P.vmax);
-    }
-    wbs = tmul(R, ww); vbs = tmul(R, vw);
-    __syncwarp();                                     // every lane has read F / H: the leg table becomes the rows' table
-    if (l16 == 0) {                                   // predicted base velocity for the rows' right-hand sides (any lane of the warp may build them)
-      envtab[kEvVel] = wbs.x; envtab[kEvVel + 1] = wbs.y; envtab[kEvVel + 2] = wbs.z;
-      envtab[kEvVel + 3] = vbs.x; envtab[kEvVel + 4] = vbs.y; envtab[kEvVel + 5] = vbs.z;
-    }
-    if (i == 0) {
-      float* lt = legtab + k * kLegW;
-#pragma unroll
-      for (int m = 0; m < 3; m++)
-#pragma unroll
-        for (int t = 0; t < 6; t++) lt[kLgW + 6 * m + t] = W[m][t];
-      lt[kLgL10] = L10; lt[kLgL20] = L20; lt[kLgL21] = L21; lt[kLgDinv] = di[0]; lt[kLgDinv + 1] = di[1]; lt[kLgDinv + 2] = di[2];
-      lt[kLgQd] = qd[0]; lt[kLgQd + 1] = qd[1]; lt[kLgQd + 2] = qd[2];
-      lt[kLgC3] = c3; lt[kLgS3] = s3;
-    }
-    }   // ================ end of the forward dynamics
     T16_MARK(1);
     __syncwarp();
     const M3 R = qmat(qp);                            // world <- B' (recomputed: cheaper than keeping nine registers alive)
@@ -1390,6 +1434,9 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
     T16_MARK(3);
     // ---------------- apply the impulses, clamp, integrate (btMultiBody::stepPositionsMultiDof)
     {
+      ww = ld3(envtab + kEvWp); vw = ld3(envtab + (kEvWp + 3));      // the predicted velocities factorise_robot left
+#pragma unroll
+      for (int t = 0; t < 3; t++) qd[t] = legtab[k * kLegW + kLgQd + t];
       V3 dw = mul(R, V3{dvb[0], dvb[1], dvb[2]}), dv = mul(R, V3{dvb[3], dvb[4], dvb[5]});
       ww = V3{clampf(ww.x + dw.x, -P.vmax, P.vmax), clampf(ww.y + dw.y, -P.vmax, P.vmax), clampf(ww.z + dw.z, -P.vmax, P.vmax)};
       vw = V3{clampf(vw.x + dv.x, -P.vmax, P.vmax), clampf(vw.y + dv.y, -P.vmax, P.vmax), clampf(vw.z + dv.z, -P.vmax, P.vmax)};
