@@ -28,6 +28,9 @@ Model refresh: `update_policy(weights)` (every worker) and `SepmcRolloutWorker.u
 worker's stream (set_weights / set_model of the handle: a host list, or a flat CUDA tensor, e.g. the blob the learner rank broadcast);
 they take effect from the next `step()`, and the LSTM states, masks, counters and slabs stay as they are: an episode in progress continues
 with the new weights.
+Several GPUs: `UnrollExchange(worker)` hands each finished unroll to the learner rank in place (the slab and the per-slab state, mask and
+bootstrap value go out of the worker's own buffers in one NCCL group); the worker's stream waits on the device for a slab's hand-over
+before it writes into that slab again.
 The recurrent levels keep their LSTM states on the device ([N, 128] at the environmental level: code LSTM, then value LSTM; [P, 192]
 for seat 0 at the strategic level: heading, code and value LSTM, and [P, 128] for seat 1), and each forward receives the done flags of
 the step before it, so a finished episode's state is wiped exactly where the reference actor's mask is set.
@@ -38,7 +41,7 @@ import torch
 
 from ..policy_epmc import DeviceHierPolicy, DeviceOpponentPool, DeviceSepmcTrainPolicy
 from .trajectory import (ACT_DIM, COL_NEGLOGP, COL_VALUE, HCOL_CODE, HCOL_NEGLOGP, HCOL_VALUE, HIER_OBS_DIM, HIER_TRAJ_WIDTH, OBS_DIM,
-                         SCOL_CODE, SCOL_HEADING, SCOL_NEGLOGP, SCOL_OPPONENT, SCOL_VALUE, SEPMC_OBS_DIM, SEPMC_TRAJ_WIDTH, TRAJ_WIDTH)
+                         SCOL_CODE, SCOL_HEADING, SCOL_NEGLOGP, SCOL_OPPONENT, SCOL_VALUE, SEPMC_OBS_DIM, SEPMC_TRAJ_WIDTH, TRAJ_WIDTH, HandOver)
 
 # what the recurrent workers' finish_unroll() returns: the [T, N, width] slab view, then the learner's state [rows, state_dim] and
 # mask [rows] (uint8) its first forward started from, and V(observation T) [rows]; all valid until the end of the NEXT unroll
@@ -66,6 +69,7 @@ class _SlabWorker:
         self.act, self.rew, self.done = self._zeros(self.n, ACT_DIM), self._zeros(self.n), self._zeros(self.n, dtype=torch.uint8)
         self.boots = [self._zeros(self.rows) for _ in range(2)]     # per slab: V(observation T)
         self.seed, self.calls = int(seed), 0
+        self.handed = [None, None]          # per slab: the event that ends its hand-over to the learner rank (UnrollExchange)
         # noise keyed by the global id of the forward's row (env or pair): equal seeds on two shards still differ
         self.gid0 = int(engine.cfg.global_env_offset) // self._SEATS
         engine.set_option("record", 2)      # a_t | r_t | done_t go to the slab row BEFORE the one receiving obs_{t+1}
@@ -112,9 +116,17 @@ class _SlabWorker:
         with torch.cuda.stream(self.stream):
             # V of the observation that follows the last record: the bootstrap of the lambda-return (unroll.py)
             self._bootstrap(done_buf[self.T], self.boots[i])
+            self._claim(1 - i)
             self.buf[0, :, :self._OBS_DIM] = done_buf[self.T, :, :self._OBS_DIM]
         self.t = 0
         return self._unroll(done_buf[:self.T], i)
+
+    def _claim(self, i):
+        # slab i (and its state, mask and bootstrap value) may still be on its way to the learner rank: the worker's stream waits for the
+        # end of that transfer before anything writes into them again (the host does not wait)
+        if self.handed[i] is not None:
+            self.stream.wait_event(self.handed[i])
+            self.handed[i] = None
 
     def wait(self):
         """Make torch's current stream wait for everything queued so far (call before reading a finished slab there)."""
@@ -299,3 +311,63 @@ class SepmcRolloutWorker(_RecurrentWorker):
         if not self.pool:
             raise ValueError("the worker plays a single opponent")
         self.opp.set_probs(probs)
+
+
+class UnrollExchange:
+    """Hands the finished unrolls of a rollout worker (any level) to the learner rank `dst` of `group`, overlapped with the next unroll.
+
+    `hand_over(u)` takes what `worker.finish_unroll()` returned and posts its transfer (`trajectory.HandOver`) on a side stream behind
+    the worker's stream: the `[T, N, W]` slab -- the leading rows of the worker's `[T+1, N, W]` buffer -- and, per slab, the recurrent
+    levels' `initial_state` and `first_mask` and every level's `bootstrap_value` (V of observation T) go out in place, in one NCCL group;
+    the host does not wait.  The finished slab stays valid during the next unroll and is written again from the end of it
+    (`finish_unroll()` puts observation T into row 0 of the other slab): the worker's stream waits there, on the device, for the
+    hand-over of that slab.  `gathered(b)` on `dst` returns one `Unroll` per rank, views of the received buffers shaped as the worker
+    returns them (the primitive level's with `initial_state` and `first_mask` None), ready for `slab_records` /
+    `slab_to_unrolls(u.slab, key, bootstrap_value=u.bootstrap_value)`, `hier_slab_records` or `sepmc_slab_records`; None on the other
+    ranks.  A world of 1 returns the worker's own views, with no copy (`own_copy=True` copies them as a learner rank of a larger world
+    copies its own unroll).
+
+    The strategic level sends the slab as the worker wrote it, both seats: the opponent's model (column 983) travels in the seat-0
+    records, and the seat-1 records double the bytes (4.13 GB per rank and unroll at T = 128, P = 4096, half of it seat 1).
+
+    Memory on the learner rank: `2 x world x bytes_per_rank` bytes of receive buffers, `bytes_per_rank` = T*N*W*4 + state + mask +
+    bootstrap, on top of the worker's own two `[T+1, N, W]` slabs.  At T = 128: PMC at N = 4096 sends 0.47 GB per rank (7.5 GB for
+    8 ranks); EPMC at N = 8192 3.93 GB (62.9 GB for 8 ranks, plus 7.9 GB of slabs: too much next to an engine on an 80 GB card), at
+    N = 4096 1.97 GB (31.4 GB for 8 ranks, plus 4.0 GB of slabs: fits on an 80 GB learner rank); SEPMC at P = 4096 4.13 GB (66.1 GB for
+    8 ranks).
+    """
+
+    def __init__(self, worker, dst=0, group=None, own_copy=None):
+        if not isinstance(worker, _SlabWorker):
+            raise ValueError("UnrollExchange hands over the unrolls of a RolloutWorker, HierRolloutWorker or SepmcRolloutWorker")
+        self.worker = worker
+        self.recurrent = isinstance(worker, _RecurrentWorker)
+        self.core = HandOver([(x.shape, x.dtype) for x in self._tensors(0)], worker.dev, dst, group, own_copy)
+        self.world, self.rank, self.dst, self.bytes_per_rank = self.core.world, self.core.rank, self.core.dst, self.core.bytes_per_rank
+
+    def _tensors(self, i):
+        w = self.worker
+        slab = w.bufs[i][:w.T]
+        return (slab, w.init_states[i], w.first_masks[i], w.boots[i]) if self.recurrent else (slab, w.boots[i])
+
+    def hand_over(self, u):
+        """`u`: what the worker's `finish_unroll()` just returned (the slab view at the primitive level, an `Unroll` at the other two).
+        Starts the transfer of that unroll; returns its slab index (pass it to `gathered` on the learner rank)."""
+        w = self.worker
+        slab = u.slab if isinstance(u, Unroll) else u
+        i = next((k for k in (0, 1) if slab.data_ptr() == w.bufs[k].data_ptr()), None)
+        if i is None or i == w._slab_index():
+            raise ValueError("hand_over() takes the unroll the worker's finish_unroll() returned last")
+        self.core.post(i, self._tensors(i), stream=w.stream)
+        w.handed[i] = self.core.sent[i]
+        return i
+
+    def gathered(self, b):
+        """Learner rank: one `Unroll` per rank of the unroll handed over as `b`, readable on torch's current stream (the wait is queued
+        there); None on the other ranks."""
+        g = self.core.gathered(b)
+        if g is None:
+            return None
+        if self.recurrent:
+            return [Unroll(*(x[r] for x in g)) for r in range(g[0].shape[0])]
+        return [Unroll(g[0][r], None, None, g[1][r]) for r in range(g[0].shape[0])]
