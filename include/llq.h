@@ -207,7 +207,12 @@ int llq_set_init_state(llq_handle h, const double* state37);
 int llq_load_model(llq_handle h, const double* blob, int64_t n_doubles);
 
 /* Replaces: MotionLib._open_all_mocap_datas (ML:19-46).  frames: [total_frames,19] float64 (clips back to
- * back, file order = sorted names), clip_offsets: [n_clips+1] prefix offsets, frame_dt = "FrameDuration". */
+ * back, file order = sorted names), clip_offsets: [n_clips+1] prefix offsets, frame_dt = "FrameDuration".
+ * Every clip needs at least margin + 3 frames (margin = ceil(policy_dt / frame_dt) + 1 / frame_dt + 2).
+ * Clip limit (CUDA engine): the reset kernel keeps the prioritized clip table in shared memory, 8 B per clip beside its static
+ * tables, so n_clips <= (cudaDevAttrMaxSharedMemoryPerBlockOptin - static shared memory of the reset kernel) / 8: 26,814 clips on an
+ * H100.  A larger table is refused with LLQ_EINVAL and a message naming the limit; the handle keeps its previous table.  The CPU
+ * oracle has no limit. */
 int llq_load_mocap(llq_handle h, const double* frames, const int32_t* clip_offsets, int32_t n_clips, double frame_dt);
 
 /* Replaces: MotionLib.obstacles_info + PrimitiveLevelEnv._create_obstacle / _update_obstacle (ML:38-42, PLE:173-193,262-268,

@@ -12,6 +12,7 @@
 #include "llq_kernels.cuh"
 #include "llq_step16.cuh"
 
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -60,7 +61,9 @@ struct llq_engine {
   bool profile = false; cudaEvent_t ev[3] = {nullptr, nullptr, nullptr}; bool ev_valid = false;
   llq::SphTable* d_sph = nullptr; llq::SphTable h_sph{};   // collision spheres of the robot (llq_step16.cuh)
   int record = 0;              // "record" option: the step kernel also writes action | reward | done behind the observation of a slab row
-  unsigned smem_attr_set = 0;  // bit 16 + ENV: cudaFuncAttributeMaxDynamicSharedMemorySize raised for that kernel instance on this handle's device
+  unsigned smem_attr_set = 0;  // bit 16 + ENV (step kernel), 20 + ENV (reset kernel): cudaFuncAttributeMaxDynamicSharedMemorySize raised for
+                               // that kernel instance on this handle's device
+  int reset_smem_optin = 0;    // > 0: the clip table needs the reset kernel's dynamic shared memory raised to this many bytes (llq_load_mocap)
 };
 
 namespace {
@@ -115,12 +118,18 @@ int ensure_scratch(llq_handle h, size_t bytes) {
 llq::MocapDev mocap_dev(llq_handle h) { return llq::MocapDev{h->d_frames, h->d_clip_off, h->n_clips, h->d_ob_table, h->d_ob_off}; }
 
 template <int ENV>
-void launch_reset_t(llq_handle h, const llq::EnvArrays& E, const llq::ResetParams& RP, float* obs2, long long ld, cudaStream_t s) {
+int launch_reset_t(llq_handle h, const llq::EnvArrays& E, const llq::ResetParams& RP, float* obs2, long long ld, cudaStream_t s) {
   constexpr int BLOCK = llq::kResetBlock;
   int threads = 4 * h->cfg.n_envs;
   int grid = (threads + BLOCK - 1) / BLOCK;
   size_t smem = sizeof(double) * (size_t)(h->n_clips > 0 ? h->n_clips : 1);
+  const unsigned bit = 1u << (20 + ENV);
+  if (h->reset_smem_optin > 0 && !(h->smem_attr_set & bit)) {
+    CK(cudaFuncSetAttribute(llq::pmc_reset_kernel<ENV>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->reset_smem_optin));
+    h->smem_attr_set |= bit;
+  }
   llq::pmc_reset_kernel<ENV><<<grid, BLOCK, smem, s>>>(E, mocap_dev(h), h->P, h->d_model, RP, obs2, ld);
+  return LLQ_OK;
 }
 template <int ENV>
 int launch_step16(llq_handle h, const llq::EnvArrays& E, const float* a, float* obs2, long long ld, cudaStream_t s) {
@@ -143,12 +152,12 @@ int launch_step(llq_handle h, const llq::EnvArrays& E, const float* a, float* ob
   if (h->cfg.env_kind == LLQ_ENV_SEPMC) return launch_step16<2>(h, E, a, obs2, ld, s);
   return epmc ? launch_step16<1>(h, E, a, obs2, ld, s) : launch_step16<0>(h, E, a, obs2, ld, s);
 }
-void launch_reset(llq_handle h, const llq::EnvArrays& E, const llq::ResetParams& RP, float* obs2, long long ld, cudaStream_t s) {
-  if (h->cfg.env_kind == LLQ_ENV_EPMC && h->cfg.element_id != 0) launch_reset_t<3>(h, E, RP, obs2, ld, s);
-  else if (h->cfg.env_kind == LLQ_ENV_EPMC) launch_reset_t<1>(h, E, RP, obs2, ld, s);
-  else if (h->cfg.env_kind == LLQ_ENV_SEPMC) launch_reset_t<2>(h, E, RP, obs2, ld, s);
-  else launch_reset_t<0>(h, E, RP, obs2, ld, s);
+int launch_reset(llq_handle h, const llq::EnvArrays& E, const llq::ResetParams& RP, float* obs2, long long ld, cudaStream_t s) {
   h->counters[4]++;
+  if (h->cfg.env_kind == LLQ_ENV_EPMC && h->cfg.element_id != 0) return launch_reset_t<3>(h, E, RP, obs2, ld, s);
+  if (h->cfg.env_kind == LLQ_ENV_EPMC) return launch_reset_t<1>(h, E, RP, obs2, ld, s);
+  if (h->cfg.env_kind == LLQ_ENV_SEPMC) return launch_reset_t<2>(h, E, RP, obs2, ld, s);
+  return launch_reset_t<0>(h, E, RP, obs2, ld, s);
 }
 
 llq::ResetParams reset_params(llq_handle h, int mode, bool update_table) {
@@ -419,11 +428,31 @@ int llq_load_mocap(llq_handle h, const double* frames, const int32_t* off, int32
   if (!h || !frames || !off || n_clips <= 0 || !(frame_dt > 0)) return fail(LLQ_EINVAL, "bad mocap arguments");
   int rc = set_device(h);
   if (rc) return rc;
-  h->frame_dt = frame_dt;
+  // The reset kernel holds the clip table (8 B per clip) in dynamic shared memory beside its static tables, so a table fits when
+  // static + 8 C bytes stays within the device's opt-in ceiling.  A refused table leaves the handle's current one in place.
+  size_t static_smem = 0;
+  for (const void* k : {(const void*)llq::pmc_reset_kernel<0>, (const void*)llq::pmc_reset_kernel<1>,
+                        (const void*)llq::pmc_reset_kernel<2>, (const void*)llq::pmc_reset_kernel<3>}) {
+    cudaFuncAttributes fa;
+    CK(cudaFuncGetAttributes(&fa, k));
+    static_smem = std::max(static_smem, fa.sharedSizeBytes);
+  }
+  int optin = 0, dflt = 0;
+  CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->cfg.device));
+  CK(cudaDeviceGetAttribute(&dflt, cudaDevAttrMaxSharedMemoryPerBlock, h->cfg.device));
+  const long long max_clips = ((long long)optin - (long long)static_smem) / (long long)sizeof(double);
+  if (n_clips > max_clips)
+    return fail(LLQ_EINVAL, "mocap table of " + std::to_string(n_clips) + " clips: the reset kernel's shared-memory clip table holds at most " +
+                            std::to_string(max_clips) + " clips on this device");
   int frame_rate = (int)(1.0 / frame_dt);                                                     // ML:34
-  h->margin = (int)std::ceil(h->cfg.policy_dt / frame_dt) + frame_rate + 2;                   // ML:35
+  const int margin = (int)std::ceil(h->cfg.policy_dt / frame_dt) + frame_rate + 2;            // ML:35
   for (int c = 0; c < n_clips; c++)
-    if (off[c + 1] - off[c] < h->margin + 3) return fail(LLQ_EINVAL, "mocap clip shorter than margin + 3 frames");
+    if (off[c + 1] - off[c] < margin + 3) return fail(LLQ_EINVAL, "mocap clip shorter than margin + 3 frames");
+  h->frame_dt = frame_dt;
+  h->margin = margin;
+  // past the default 48 kB per block the reset kernel launches only with the opt-in raised; every handle raises it to the same
+  // ceiling, so handles with different tables on one device never lower it under one another
+  h->reset_smem_optin = static_smem + sizeof(double) * (size_t)n_clips > (size_t)dflt ? optin - (int)static_smem : 0;
   h->n_clips = n_clips;
   h->clip_off.assign(off, off + n_clips + 1);
   const size_t total = (size_t)off[n_clips];
@@ -504,7 +533,8 @@ static int do_reset(llq_handle h, const uint8_t* mask, const int32_t* clip, cons
     CK(cudaMemcpyAsync(h->d_clip_in, hc, n * sizeof(int), cudaMemcpyHostToDevice, h->stream));
     RP.clip_in = h->d_clip_in; RP.time_in = h->d_time_in;
   }
-  launch_reset(h, h->E, RP, nullptr, h->obs_dim, h->stream);
+  int rc = launch_reset(h, h->E, RP, nullptr, h->obs_dim, h->stream);
+  if (rc) return rc;
   CK(cudaGetLastError());
   if (obs) CK(cudaMemcpyAsync(h->h_obs, h->E.obs, sizeof(float) * h->obs_dim * n, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
@@ -563,7 +593,8 @@ int llq_step_ex(llq_handle h, const float* actions, float* obs, int64_t obs_ld, 
   if (h->profile) CK(cudaEventRecord(h->ev[1], s));
   // prioritized-sampling table update (PLE:235-240) + auto reset of finished envs
   llq::ResetParams RP = reset_params(h, h->cfg.auto_reset ? 0 : 3, true);
-  launch_reset(h, E, RP, obs2, (long long)obs_ld, s);
+  rc = launch_reset(h, E, RP, obs2, (long long)obs_ld, s);
+  if (rc) return rc;
   if (h->profile) { CK(cudaEventRecord(h->ev[2], s)); h->ev_valid = true; }
   h->parity ^= 1;
   CK(cudaGetLastError());

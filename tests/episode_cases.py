@@ -76,9 +76,9 @@ TERMS = ("jp", "jv", "ee", "pose", "vel")
 
 
 # ------------------------------------------------------------------------------------------------------------ mocap and geometry
-def mocap(n_clips):
-    """synthetic clips of 300..420 frames, the base pitched by TILT; with their plate table"""
-    mc = synthetic_mocap(n_clips, seed=n_clips, min_frames=300, max_frames=420)
+def mocap(n_clips, frames=(300, 420)):
+    """synthetic clips of frames[0]..frames[1] frames, the base pitched by TILT; with their plate table"""
+    mc = synthetic_mocap(n_clips, seed=n_clips, min_frames=frames[0], max_frames=frames[1])
     f = mc.frames.copy()
     f[:, 3:7] = (R.from_quat(f[:, 3:7]) * R.from_euler("y", TILT)).as_quat()
     mc = MocapTable(f, mc.offsets, mc.frame_dt, mc.names)
@@ -316,8 +316,7 @@ def uniforms(seed, gid, ep):
 def draw(ctx, cdf, gid, ep):
     """(clip, t0, cursor, fraction) of the auto-reset of envs with global ids gid and episode ids ep"""
     u1, u2 = uniforms(ctx["seed"], gid, ep)
-    above = cdf[None, :] > u1[:, None]
-    clip = np.where(above.any(1), np.argmax(above, 1), len(cdf) - 1)
+    clip = np.minimum(np.searchsorted(cdf, u1, side="right"), len(cdf) - 1)      # the first clip with cdf > u1; none: the last
     nf, m, dt = ctx["nf"][clip], ctx["m"], ctx["mc"].frame_dt
     t0 = u2 * (dt * (nf - m - 1).astype(np.float64))
     fid = np.floor(t0 / dt).astype(np.int64)
@@ -345,9 +344,9 @@ def reset_sensitivity(ctx, clip, fid, frac, draws=R_DRAWS):
 
 
 # ------------------------------------------------------------------------------------------------------------ designed batches
-def context(case):
+def context(case, frames=(300, 420)):
     n, n_clips, substeps, factor, gid0, weights = case
-    mc, (ob_table, ob_off) = mocap(n_clips)
+    mc, (ob_table, ob_off) = mocap(n_clips, frames)
     nf = np.diff(mc.offsets).astype(np.int64)
     return dict(n=n, mc=mc, frames=stored_frames(mc), off=mc.offsets.astype(np.int64), nf=nf, m=margin(mc.frame_dt), substeps=substeps,
                 sim_dt=1.0 / 500.0, factor=factor, gid0=gid0, weights=weights, seed=SEED + n, ob_table=ob_table, ob_off=ob_off,
@@ -568,10 +567,11 @@ def _exact_end_time(ctx, T):
     return t0
 
 
-def design_edges(ctx, before, ref, rng, n_inner=6):
+def design_edges(ctx, before, ref, rng, n_inner=6, targets=()):
     """F_AVG_REWARD to set before the step.  Clips without a finisher are free: a free pair (j, j + 1) is re-weighted so that cdf[j]
     lands 1e-8..1e-6 above or below the u1 of a finishing env -- the smallest u1 on the first edge, the largest on the last one, and
-    up to n_inner others on the edge they fall next to.  Returns the table and {env: (edge clip j, side)}."""
+    up to n_inner others on the edge they fall next to, or on the edges `targets` names, in order.  Returns the table and
+    {env: (edge clip j, side)}."""
     C = ctx["mc"].n_clips
     avg = before["avg"].copy()
     done = ref["done"]
@@ -582,10 +582,22 @@ def design_edges(ctx, before, ref, rng, n_inner=6):
     busy = set(int(c) for c in before["clip"][fin])
     f = ctx["factor"]
     order = [int(np.argmin(u1)), int(np.argmax(u1))] + [k for k in rng.permutation(len(fin)) if k not in (np.argmin(u1), np.argmax(u1))]
+    if len(targets):              # the target edges (increasing) take finishers with increasing u1, each the one nearest below its
+        cdf0 = table(ctx, done, before["clip"], ref["reward_sum"], avg)[2]       # cdf: its pair then grows by little
+        rest = sorted(order[2:], key=lambda k: u1[k])
+        pick = []
+        for i, j in enumerate(targets):
+            cand = rest[:len(rest) - (len(targets) - 1 - i)]
+            if not cand:
+                break
+            k = min(cand, key=lambda k: (u1[k] > cdf0[j], abs(cdf0[j] - u1[k])))
+            pick.append(k)
+            rest = rest[rest.index(k) + 1:]
+        order = order[:2] + pick + [k for k in order[2:] if k not in pick]
     plan, used = [], set()
     for r, k in enumerate(order):
         upd, _, cdf, _ = table(ctx, done, before["clip"], ref["reward_sum"], avg)
-        j = 0 if r == 0 else (C - 2 if r == 1 else int(np.searchsorted(cdf, u1[k], side="right")))
+        j = 0 if r == 0 else (C - 2 if r == 1 else (targets[r - 2] if r - 2 < len(targets) else int(np.searchsorted(cdf, u1[k], side="right"))))
         if j >= C - 1 or {j, j + 1} & (busy | used):
             continue
         side = 1.0 if r % 2 == 0 else -1.0
@@ -782,15 +794,29 @@ def ulps(a, b):
     return np.abs(a.view(np.int64) - b.view(np.int64))
 
 
+def reset_ratios(ctx, state, kin, obs, clip, fid, frac, kappa=KAPPA):
+    """the state, F_KIN_STATE and observation rows of envs reset at (clip, cursor, fraction) against the statement; returns the
+    largest error / S ratios"""
+    rst, robs, Ss, So = reset_sensitivity(ctx, clip, fid, frac)
+    ratios = {}
+    got = state.astype(np.float64); got[:, 3:7] = _sign_fix(got[:, 3:7], rst[:, 3:7])
+    ratios["reset_state"] = _ratio(got, rst, Ss, kappa, "reset state")
+    got = kin.astype(np.float64); got[:, 3:7] = _sign_fix(got[:, 3:7], rst[:, 3:7])
+    ratios["reset_kin"] = _ratio(got, rst, Ss, kappa, "reset F_KIN_STATE")
+    ratios["reset_obs"] = _ratio(obs, robs, So, kappa, "reset obs")
+    return ratios
+
+
 def run_case(lib, k, io="host", kappa=KAPPA, oracle=False):
-    """Run batch k through `lib` (CUDA engine or oracle) and compare every output with the statement.  Engine A (auto_reset 0)
+    """Run batch k (an index of CASES, or a batch (ctx, before, categories, designed) built elsewhere) through `lib` (CUDA engine or
+    oracle) and compare every output with the statement.  Engine A (auto_reset 0)
     takes two steps, the second with the highest finisher of every clip taken back (the winner ping-pong buffers); engine B
     (auto_reset 1) takes the first step again and draws.  Returns the largest error / S ratios.
 
     oracle=True: the oracle keeps reward_sum in fp64 (the reference's python float), the engine in fp32.  Its rewards are held to
     5e-7 + 4 S, its reward sums and table to 1e-6 relative, and the draws of the designed-edge envs (which lie closer to an edge than that
     difference moves it) are not compared."""
-    ctx, before, cats, designed = case(k)
+    ctx, before, cats, designed = case(k) if isinstance(k, int) else k
     n = ctx["n"]
     ratios = {}
     A, B = make(lib, ctx, 0), make(lib, ctx, 1)
@@ -857,12 +883,7 @@ def run_case(lib, k, io="host", kappa=KAPPA, oracle=False):
             assert np.array_equal(fb["clip"][fin], clip), [(int(fin[i]), int(fb["clip"][fin][i]), int(clip[i])) for i in np.nonzero(fb["clip"][fin] != clip)[0][:6]]
             assert np.array_equal(fb["time"][fin], t0) and np.array_equal(fb["episode"][fin], before["episode"][fin] + 1)
             assert np.all(fb["ob_id"][fin] == 0) and np.all(fb["reward_sum"][fin] == 0)
-            rst, robs, Ss, So = reset_sensitivity(ctx, clip, fid, frac)
-            got = fb["state"][fin].astype(np.float64); got[:, 3:7] = _sign_fix(got[:, 3:7], rst[:, 3:7])
-            ratios["reset_state"] = _ratio(got, rst, Ss, kappa, "reset state")
-            got = fb["kin"][fin].astype(np.float64); got[:, 3:7] = _sign_fix(got[:, 3:7], rst[:, 3:7])
-            ratios["reset_kin"] = _ratio(got, rst, Ss, kappa, "reset F_KIN_STATE")
-            ratios["reset_obs"] = _ratio(oB[fin], robs, So, kappa, "reset obs")
+            ratios.update(reset_ratios(ctx, fb["state"][fin], fb["kin"][fin], oB[fin], clip, fid, frac, kappa))
             assert np.array_equal(oB[fin], fb["obs"][fin])
             assert np.all(oB[fin][:, 99:135] == 0) and np.array_equal(oB[fin][:, 0:33], oB[fin][:, 66:99])
         # ---- record columns: the finishing step's action, reward and done, also for envs that were reset in the same call
