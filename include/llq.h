@@ -99,7 +99,7 @@ extern "C" {
 #define LLQ_F_REWARD_SUM  3  /* float   [N]     PLE.reward_sum (PLE:231) */
 #define LLQ_F_EPISODE_STEPS 4 /* int32  [N]     PLE._episode_steps (PLE:197) */
 #define LLQ_MAX_SPHERES   32 /* collision spheres of the robot: 4 feet, 4 knee wheels, 4 hips, 4 thighs, 8 shank, 8 trunk corners */
-#define LLQ_MAX_CONTACTS  8  /* manifold points kept per robot and sub-step (sphere order); counter [5] counts what was dropped */
+#define LLQ_MAX_CONTACTS  8  /* manifold points kept per robot and sub-step (sphere order); counter LLQ_CNT_DROPPED counts what was dropped */
 #define LLQ_MAX_LIMIT_ROWS 8 /* joint-limit rows kept per robot and sub-step (joint order) */
 #define LLQ_F_WARMSTART   5  /* float   [N,32]  previous sub-step's normal impulse per collision sphere (contact warm start) */
 #define LLQ_F_OBS         6  /* float   [N,207] last observation (carries the 3-frame prop / action history) */
@@ -250,9 +250,13 @@ int llq_step_ex(llq_handle h, const float* actions, float* obs, int64_t obs_ld, 
 int llq_get_field(llq_handle h, int field, void* dst);
 int llq_set_field(llq_handle h, int field, const void* src);
 
-/* counters: [0] env steps, [1] episodes finished, [2] contact rows solved, [3] joint-limit rows solved,
- * [4] kernel launches issued by the engine (CUDA) / 0 (CPU), [5] manifold points / limit rows dropped by the LLQ_MAX_CONTACTS /
- * LLQ_MAX_LIMIT_ROWS caps. n <= 8. */
+/* counters: out[LLQ_CNT_*] below, n <= 8. */
+#define LLQ_CNT_ENV_STEPS     0   /* env steps */
+#define LLQ_CNT_EPISODES      1   /* episodes finished */
+#define LLQ_CNT_CONTACT_ROWS  2   /* contact rows solved */
+#define LLQ_CNT_LIMIT_ROWS    3   /* joint-limit rows solved */
+#define LLQ_CNT_LAUNCHES      4   /* kernel launches issued by the engine (CUDA) / 0 (CPU) */
+#define LLQ_CNT_DROPPED       5   /* manifold points / limit rows dropped by the LLQ_MAX_CONTACTS / LLQ_MAX_LIMIT_ROWS caps */
 int llq_get_counters(llq_handle h, int64_t* out, int32_t n);
 
 /* Per-kernel device timing of the most recent llq_step*: out[0] = fused step kernel ms, out[1] = reset/table kernel ms

@@ -25,6 +25,8 @@ AUX_COUNTER, AUX_TOTAL_SPD, AUX_MAX_SPD, AUX_PUSH_COUNT, AUX_PUSH_F, AUX_FOOT_FR
  AUX_INIT_POS_DIFF_LEN) = 1, 2, 3, 4, 5, 6, 15, 17
 (AUX_WITH_FLAG, AUX_FLAG_X, AUX_FLAG_Y, AUX_CONTROL_SPD, AUX_OPPO_VISIBLE, AUX_SWITCH_FLAG, AUX_FLAG_DRAWS,
  AUX_FLAG_TOUCH) = 1, 2, 3, 4, 5, 6, 15, 17
+# VecEngine.counters() slots (LLQ_CNT_* of include/llq.h)
+CNT_ENV_STEPS, CNT_EPISODES, CNT_CONTACT_ROWS, CNT_LIMIT_ROWS, CNT_LAUNCHES, CNT_DROPPED = range(6)
 
 # field id -> (dtype, per-env width or None for per-clip tables)
 _FIELDS = {

@@ -19,6 +19,7 @@
 #include <cstring>
 #include <new>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 namespace {
@@ -45,7 +46,7 @@ struct llq_engine {
   std::vector<int> clip_off;
   llq::EnvArrays E{};
   float* d_actions = nullptr;
-  int obs_dim = LLQ_OBS_DIM; bool has_init_state = false; llq::ModelConst h_model{};
+  int instance = llq::kPmc; int obs_dim = LLQ_OBS_DIM; bool has_init_state = false; llq::ModelConst h_model{};
   int* d_winner[2] = {nullptr, nullptr};
   double* d_avg[2] = {nullptr, nullptr};
   double* d_prob = nullptr; double* d_max_steps = nullptr;
@@ -61,8 +62,7 @@ struct llq_engine {
   bool profile = false; cudaEvent_t ev[3] = {nullptr, nullptr, nullptr}; bool ev_valid = false;
   llq::SphTable* d_sph = nullptr; llq::SphTable h_sph{};   // collision spheres of the robot (llq_step16.cuh)
   int record = 0;              // "record" option: the step kernel also writes action | reward | done behind the observation of a slab row
-  unsigned smem_attr_set = 0;  // bit 16 + ENV (step kernel), 20 + ENV (reset kernel): cudaFuncAttributeMaxDynamicSharedMemorySize raised for
-                               // that kernel instance on this handle's device
+  bool step_smem_raised = false, reset_smem_raised = false;   // cudaFuncAttributeMaxDynamicSharedMemorySize raised for that kernel
   int reset_smem_optin = 0;    // > 0: the clip table needs the reset kernel's dynamic shared memory raised to this many bytes (llq_load_mocap)
 };
 
@@ -117,47 +117,50 @@ int ensure_scratch(llq_handle h, size_t bytes) {
 
 llq::MocapDev mocap_dev(llq_handle h) { return llq::MocapDev{h->d_frames, h->d_clip_off, h->n_clips, h->d_ob_table, h->d_ob_off}; }
 
-template <int ENV>
-int launch_reset_t(llq_handle h, const llq::EnvArrays& E, const llq::ResetParams& RP, float* obs2, long long ld, cudaStream_t s) {
+// The kernel instance (llq_kernels.cuh) a configuration runs; -1: an EPMC element_id outside 0..3
+int kernel_instance(const llq_config& c) {
+  if (c.env_kind != LLQ_ENV_EPMC) return c.env_kind == LLQ_ENV_SEPMC ? llq::kSepmc : llq::kPmc;
+  return c.element_id == 0 ? llq::kEpmc : (c.element_id >= 1 && c.element_id <= 3 ? llq::kCorridor : -1);
+}
+// f(std::integral_constant<int, ENV>()) for the kernel instance ENV = instance
+template <typename F> int with_instance(int instance, F f) {
+  switch (instance) {
+    case llq::kEpmc: return f(std::integral_constant<int, llq::kEpmc>());
+    case llq::kSepmc: return f(std::integral_constant<int, llq::kSepmc>());
+    case llq::kCorridor: return f(std::integral_constant<int, llq::kCorridor>());
+    default: return f(std::integral_constant<int, llq::kPmc>());
+  }
+}
+// every launch: counted; when smem_limit > 0, the kernel's dynamic shared memory limit is raised to it once per handle (`raised`)
+int before_launch(llq_handle h, const void* kernel, int smem_limit, bool& raised) {
+  h->counters[LLQ_CNT_LAUNCHES]++;
+  if (smem_limit > 0 && !raised) CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_limit));
+  raised = raised || smem_limit > 0;
+  return LLQ_OK;
+}
+int launch_reset(llq_handle h, const llq::EnvArrays& E, const llq::ResetParams& RP, float* obs2, long long ld, cudaStream_t s) {
   constexpr int BLOCK = llq::kResetBlock;
   int threads = 4 * h->cfg.n_envs;
   int grid = (threads + BLOCK - 1) / BLOCK;
   size_t smem = sizeof(double) * (size_t)(h->n_clips > 0 ? h->n_clips : 1);
-  const unsigned bit = 1u << (20 + ENV);
-  if (h->reset_smem_optin > 0 && !(h->smem_attr_set & bit)) {
-    CK(cudaFuncSetAttribute(llq::pmc_reset_kernel<ENV>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->reset_smem_optin));
-    h->smem_attr_set |= bit;
-  }
-  llq::pmc_reset_kernel<ENV><<<grid, BLOCK, smem, s>>>(E, mocap_dev(h), h->P, h->d_model, RP, obs2, ld);
-  return LLQ_OK;
+  return with_instance(h->instance, [&](auto env) {
+    const auto kernel = llq::pmc_reset_kernel<decltype(env)::value>;
+    if (const int rc = before_launch(h, (const void*)kernel, h->reset_smem_optin, h->reset_smem_raised)) return rc;
+    kernel<<<grid, BLOCK, smem, s>>>(E, mocap_dev(h), h->P, h->d_model, RP, obs2, ld);
+    return LLQ_OK;
+  });
 }
-template <int ENV>
-int launch_step16(llq_handle h, const llq::EnvArrays& E, const float* a, float* obs2, long long ld, cudaStream_t s) {
+int launch_step(llq_handle h, const llq::EnvArrays& E, const float* a, float* obs2, long long ld, cudaStream_t s) {
   constexpr int EPB = LLQ16_BLOCK / 16;           // envs per CTA (16 lanes each)
   const int grid = (h->cfg.n_envs + EPB - 1) / EPB;
   const size_t smem = sizeof(float) * (EPB * llq::kEnvFloats + (LLQ16_BLOCK / 32) * llq::kATabWarp);
-  const unsigned bit = 1u << (16 + ENV);          // static + dynamic shared memory exceeds 48 kB: per-device opt-in, once per handle
-  if (!(h->smem_attr_set & bit)) {
-    CK(cudaFuncSetAttribute(llq::llq_step16_kernel<ENV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    h->smem_attr_set |= bit;
-  }
-  llq::llq_step16_kernel<ENV><<<grid, LLQ16_BLOCK, smem, s>>>(E, mocap_dev(h), h->P, h->d_model, h->d_sph, a, obs2, ld, h->d_winner[h->parity],
-                                                   (unsigned long long)h->cfg.seed, (long long)h->cfg.global_env_offset, h->record);
-  return LLQ_OK;
-}
-int launch_step(llq_handle h, const llq::EnvArrays& E, const float* a, float* obs2, long long ld, cudaStream_t s) {
-  const bool epmc = h->cfg.env_kind == LLQ_ENV_EPMC;
-  h->counters[4]++;
-  if (epmc && h->cfg.element_id != 0) return launch_step16<3>(h, E, a, obs2, ld, s);      // corridor arenas: the box-aware instance
-  if (h->cfg.env_kind == LLQ_ENV_SEPMC) return launch_step16<2>(h, E, a, obs2, ld, s);
-  return epmc ? launch_step16<1>(h, E, a, obs2, ld, s) : launch_step16<0>(h, E, a, obs2, ld, s);
-}
-int launch_reset(llq_handle h, const llq::EnvArrays& E, const llq::ResetParams& RP, float* obs2, long long ld, cudaStream_t s) {
-  h->counters[4]++;
-  if (h->cfg.env_kind == LLQ_ENV_EPMC && h->cfg.element_id != 0) return launch_reset_t<3>(h, E, RP, obs2, ld, s);
-  if (h->cfg.env_kind == LLQ_ENV_EPMC) return launch_reset_t<1>(h, E, RP, obs2, ld, s);
-  if (h->cfg.env_kind == LLQ_ENV_SEPMC) return launch_reset_t<2>(h, E, RP, obs2, ld, s);
-  return launch_reset_t<0>(h, E, RP, obs2, ld, s);
+  return with_instance(h->instance, [&](auto env) {
+    const auto kernel = llq::llq_step16_kernel<decltype(env)::value>;
+    if (const int rc = before_launch(h, (const void*)kernel, (int)smem, h->step_smem_raised)) return rc;   // static + dynamic > 48 kB: opt-in
+    kernel<<<grid, LLQ16_BLOCK, smem, s>>>(E, mocap_dev(h), h->P, h->d_model, h->d_sph, a, obs2, ld, h->d_winner[h->parity],
+                                           (unsigned long long)h->cfg.seed, (long long)h->cfg.global_env_offset, h->record);
+    return LLQ_OK;
+  });
 }
 
 llq::ResetParams reset_params(llq_handle h, int mode, bool update_table) {
@@ -244,7 +247,8 @@ int llq_create(const llq_config* cfg, llq_handle* out) {
   if (cfg->env_kind == LLQ_ENV_EPMC && (cfg->max_steps <= 0 || cfg->cmd_freq_hi <= cfg->cmd_freq_lo || cfg->cmd_freq_lo <= 0 ||
                                         cfg->push_interval_steps <= 0))
     return fail(LLQ_EINVAL, "bad EPMC configuration");
-  if (cfg->env_kind == LLQ_ENV_EPMC && (cfg->element_id < 0 || cfg->element_id > 3)) return fail(LLQ_EINVAL, "EPMC element_id must be 0..3");
+  const int instance = kernel_instance(*cfg);
+  if (instance < 0) return fail(LLQ_EINVAL, "EPMC element_id must be 0..3");
   if (cfg->knee_contacts < 0 || cfg->knee_contacts > 2) return fail(LLQ_EINVAL, "knee_contacts must be 0, 1 or 2");
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
@@ -253,7 +257,8 @@ int llq_create(const llq_config* cfg, llq_handle* out) {
   llq_engine* h = new (std::nothrow) llq_engine();
   if (!h) return fail(LLQ_ENOMEM, "out of memory");
   h->cfg = *cfg;
-  h->obs_dim = cfg->env_kind == LLQ_ENV_EPMC ? LLQ_OBS_DIM_EPMC : (cfg->env_kind == LLQ_ENV_SEPMC ? LLQ_OBS_DIM_SEPMC : LLQ_OBS_DIM);
+  h->instance = instance;
+  h->obs_dim = llq::obs_width(instance);
   int rc = set_device(h);
   if (rc) { delete h; return rc; }
   const size_t n = (size_t)cfg->n_envs;
@@ -261,14 +266,14 @@ int llq_create(const llq_config* cfg, llq_handle* out) {
   cudaError_t ce = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking);
   if (ce != cudaSuccess) { delete h; return fail(LLQ_ECUDA, cudaGetErrorString(ce)); }
   TRY(dalloc(&h->d_model, 1)); TRY(dalloc(&h->d_sph, 1));
-  TRY(dalloc(&h->E.pos, 3 * n)); TRY(dalloc(&h->E.st, 34 * n)); TRY(dalloc(&h->E.time, n)); TRY(dalloc(&h->E.clip, n));
+  TRY(dalloc(&h->E.pos, 3 * n)); TRY(dalloc(&h->E.st, llq::kStRows * n)); TRY(dalloc(&h->E.time, n)); TRY(dalloc(&h->E.clip, n));
   TRY(dalloc(&h->E.reward_sum, n)); TRY(dalloc(&h->E.episode_steps, n)); TRY(dalloc(&h->E.episode, n));
-  TRY(dalloc(&h->E.warm, LLQ_MAX_SPHERES * n)); TRY(dalloc(&h->E.obs, (size_t)h->obs_dim * n)); TRY(dalloc(&h->E.kin, 37 * n));
+  TRY(dalloc(&h->E.warm, LLQ_MAX_SPHERES * n)); TRY(dalloc(&h->E.obs, (size_t)h->obs_dim * n)); TRY(dalloc(&h->E.kin, LLQ_STATE_DIM * n));
   TRY(dalloc(&h->E.foot_pos, 12 * n)); TRY(dalloc(&h->E.done_reward, n)); TRY(dalloc(&h->E.done, n)); TRY(dalloc(&h->E.reward, n));
   TRY(dalloc(&h->E.counters, 8));
   TRY(dalloc(&h->E.aux, (size_t)LLQ_AUX_DIM * n));
   TRY(dalloc(&h->E.ob_id, n));
-  TRY(dalloc(&h->E.boxes, (size_t)6 * LLQ_MAX_BOXES * n)); TRY(dalloc(&h->E.nbox, n));
+  TRY(dalloc(&h->E.boxes, (size_t)llq::kBoxW * LLQ_MAX_BOXES * n)); TRY(dalloc(&h->E.nbox, n));
   TRY(dalloc(&h->d_actions, (size_t)LLQ_ACTION_DIM * n));
   TRY(dalloc(&h->d_mask, n)); TRY(dalloc(&h->d_clip_in, n)); TRY(dalloc(&h->d_time_in, n));
   ce = cudaMallocHost((void**)&h->h_actions, sizeof(float) * LLQ_ACTION_DIM * n);
@@ -405,7 +410,7 @@ int llq_load_model(llq_handle h, const double* b, int64_t n) {
     if (nfoot != 4) return fail(LLQ_EINVAL, "model blob must list the four foot spheres first");
     CK(cudaMemcpy(h->d_sph, &T, sizeof(T), cudaMemcpyHostToDevice));
   }
-  for (int i = 0; i < 37; i++) M.init_state[i] = h->h_model.init_state[i];
+  for (int i = 0; i < LLQ_STATE_DIM; i++) M.init_state[i] = h->h_model.init_state[i];
   h->h_model = M;
   CK(cudaMemcpy(h->d_model, &M, sizeof(M), cudaMemcpyHostToDevice));
   h->has_model = true;
@@ -418,7 +423,7 @@ int llq_set_init_state(llq_handle h, const double* st) {
   if (!h || !st) return fail(LLQ_EINVAL, "null argument");
   int rc = set_device(h);
   if (rc) return rc;
-  for (int i = 0; i < 37; i++) h->h_model.init_state[i] = (float)st[i];
+  for (int i = 0; i < LLQ_STATE_DIM; i++) h->h_model.init_state[i] = (float)st[i];
   if (h->has_model) CK(cudaMemcpy(h->d_model, &h->h_model, sizeof(h->h_model), cudaMemcpyHostToDevice));
   h->has_init_state = true;
   return LLQ_OK;
@@ -430,13 +435,10 @@ int llq_load_mocap(llq_handle h, const double* frames, const int32_t* off, int32
   if (rc) return rc;
   // The reset kernel holds the clip table (8 B per clip) in dynamic shared memory beside its static tables, so a table fits when
   // static + 8 C bytes stays within the device's opt-in ceiling.  A refused table leaves the handle's current one in place.
-  size_t static_smem = 0;
-  for (const void* k : {(const void*)llq::pmc_reset_kernel<0>, (const void*)llq::pmc_reset_kernel<1>,
-                        (const void*)llq::pmc_reset_kernel<2>, (const void*)llq::pmc_reset_kernel<3>}) {
-    cudaFuncAttributes fa;
-    CK(cudaFuncGetAttributes(&fa, k));
-    static_smem = std::max(static_smem, fa.sharedSizeBytes);
-  }
+  cudaFuncAttributes fa;
+  rc = with_instance(h->instance, [&](auto env) { CK(cudaFuncGetAttributes(&fa, (const void*)llq::pmc_reset_kernel<decltype(env)::value>)); return LLQ_OK; });
+  if (rc) return rc;
+  const size_t static_smem = fa.sharedSizeBytes;
   int optin = 0, dflt = 0;
   CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->cfg.device));
   CK(cudaDeviceGetAttribute(&dflt, cudaDevAttrMaxSharedMemoryPerBlock, h->cfg.device));
@@ -598,7 +600,7 @@ int llq_step_ex(llq_handle h, const float* actions, float* obs, int64_t obs_ld, 
   if (h->profile) { CK(cudaEventRecord(h->ev[2], s)); h->ev_valid = true; }
   h->parity ^= 1;
   CK(cudaGetLastError());
-  h->counters[0] += (int64_t)n;
+  h->counters[LLQ_CNT_ENV_STEPS] += (int64_t)n;
   if (io_mode == LLQ_IO_HOST) {
     if (obs) CK(cudaMemcpyAsync(h->h_obs, h->E.obs, sizeof(float) * od * n, cudaMemcpyDeviceToHost, s));
     if (reward) CK(cudaMemcpyAsync(h->h_reward, h->E.reward, sizeof(float) * n, cudaMemcpyDeviceToHost, s));
@@ -635,19 +637,19 @@ int llq_get_field(llq_handle h, int field, void* dst) {
   CK(cudaStreamSynchronize(h->stream));
   switch (field) {
     case LLQ_F_STATE: {
-      std::vector<float> tmp(34 * n);
-      rc = get_soa_f(h, h->E.st, 34, tmp.data());
+      std::vector<float> tmp(llq::kStRows * n);
+      rc = get_soa_f(h, h->E.st, llq::kStRows, tmp.data());
       if (rc) return rc;
       std::vector<double> pos(3 * n);
       CK(cudaMemcpy(pos.data(), h->E.pos, sizeof(double) * 3 * n, cudaMemcpyDeviceToHost));
       float* o = (float*)dst;
       for (size_t i = 0; i < n; i++) {
-        for (int t = 0; t < 3; t++) o[i * 37 + t] = (float)pos[t * n + i];
-        for (int t = 0; t < 34; t++) o[i * 37 + 3 + t] = tmp[i * 34 + t];
+        for (int t = 0; t < 3; t++) o[i * LLQ_STATE_DIM + llq::kStatePos + t] = (float)pos[t * n + i];
+        for (int t = 0; t < llq::kStRows; t++) o[i * LLQ_STATE_DIM + llq::kStateQuat + t] = tmp[i * llq::kStRows + t];
       }
       return LLQ_OK;
     }
-    case LLQ_F_KIN_STATE: return get_soa_f(h, h->E.kin, 37, (float*)dst);
+    case LLQ_F_KIN_STATE: return get_soa_f(h, h->E.kin, LLQ_STATE_DIM, (float*)dst);
     case LLQ_F_WARMSTART: return get_soa_f(h, h->E.warm, LLQ_MAX_SPHERES, (float*)dst);
     case LLQ_F_FOOT_POS: return get_soa_f(h, h->E.foot_pos, 12, (float*)dst);
     case LLQ_F_CLIP: CK(cudaMemcpy(dst, h->E.clip, sizeof(int) * n, cudaMemcpyDeviceToHost)); return LLQ_OK;
@@ -659,10 +661,10 @@ int llq_get_field(llq_handle h, int field, void* dst) {
     case LLQ_F_OBS: CK(cudaMemcpy(dst, h->E.obs, sizeof(float) * h->obs_dim * n, cudaMemcpyDeviceToHost)); return LLQ_OK;
     case LLQ_F_BOXES: {
       std::vector<int> nb(n);
-      CK(cudaMemcpy(dst, h->E.boxes, sizeof(float) * 6 * LLQ_MAX_BOXES * n, cudaMemcpyDeviceToHost));
+      CK(cudaMemcpy(dst, h->E.boxes, sizeof(float) * llq::kBoxW * LLQ_MAX_BOXES * n, cudaMemcpyDeviceToHost));
       CK(cudaMemcpy(nb.data(), h->E.nbox, sizeof(int) * n, cudaMemcpyDeviceToHost));
       for (size_t i = 0; i < n; i++)                      // rows past the env's box count hold stale boxes of earlier episodes
-        for (int b = nb[i]; b < LLQ_MAX_BOXES; b++) std::memset((float*)dst + (i * LLQ_MAX_BOXES + b) * 6, 0, 6 * sizeof(float));
+        for (int b = nb[i]; b < LLQ_MAX_BOXES; b++) std::memset((float*)dst + (i * LLQ_MAX_BOXES + b) * llq::kBoxW, 0, llq::kBoxW * sizeof(float));
       return LLQ_OK;
     }
     case LLQ_F_NBOX: CK(cudaMemcpy(dst, h->E.nbox, sizeof(int) * n, cudaMemcpyDeviceToHost)); return LLQ_OK;
@@ -670,10 +672,8 @@ int llq_get_field(llq_handle h, int field, void* dst) {
       std::vector<double> tmp((size_t)LLQ_AUX_DIM * n);
       CK(cudaMemcpy(tmp.data(), h->E.aux, sizeof(double) * LLQ_AUX_DIM * n, cudaMemcpyDeviceToHost));
       double* o = (double*)dst;
-      for (size_t i = 0; i < n; i++) {
+      for (size_t i = 0; i < n; i++)
         for (int t = 0; t < LLQ_AUX_DIM; t++) o[i * LLQ_AUX_DIM + t] = tmp[(size_t)t * n + i];
-        o[i * LLQ_AUX_DIM + 13] = tmp[13 * n + i];
-      }
       return LLQ_OK;
     }
     case LLQ_F_SAMPLE_PROB:
@@ -695,12 +695,12 @@ int llq_set_field(llq_handle h, int field, const void* src) {
   switch (field) {
     case LLQ_F_STATE: {
       const float* s = (const float*)src;
-      std::vector<float> st(34 * n); std::vector<double> pos(3 * n);
+      std::vector<float> st(llq::kStRows * n); std::vector<double> pos(3 * n);
       for (size_t i = 0; i < n; i++) {
-        for (int t = 0; t < 3; t++) pos[t * n + i] = (double)s[i * 37 + t];
-        for (int t = 0; t < 34; t++) st[t * n + i] = s[i * 37 + 3 + t];
+        for (int t = 0; t < 3; t++) pos[t * n + i] = (double)s[i * LLQ_STATE_DIM + llq::kStatePos + t];
+        for (int t = 0; t < llq::kStRows; t++) st[t * n + i] = s[i * LLQ_STATE_DIM + llq::kStateQuat + t];
       }
-      CK(cudaMemcpy(h->E.st, st.data(), sizeof(float) * 34 * n, cudaMemcpyHostToDevice));
+      CK(cudaMemcpy(h->E.st, st.data(), sizeof(float) * llq::kStRows * n, cudaMemcpyHostToDevice));
       CK(cudaMemcpy(h->E.pos, pos.data(), sizeof(double) * 3 * n, cudaMemcpyHostToDevice));
       return LLQ_OK;
     }
@@ -754,7 +754,7 @@ int llq_get_counters(llq_handle h, int64_t* out, int32_t n) {
   CK(cudaMemcpy(dc, h->E.counters, sizeof(dc), cudaMemcpyDeviceToHost));
   int64_t c[8];
   for (int i = 0; i < 8; i++) c[i] = h->counters[i];
-  c[1] = (int64_t)dc[1]; c[2] = (int64_t)dc[2]; c[3] = (int64_t)dc[3]; c[5] = (int64_t)dc[5];
+  for (int i : {LLQ_CNT_EPISODES, LLQ_CNT_CONTACT_ROWS, LLQ_CNT_LIMIT_ROWS, LLQ_CNT_DROPPED}) c[i] = (int64_t)dc[i];   // counted on the device
   for (int i = 0; i < n; i++) out[i] = c[i];
   return LLQ_OK;
 }

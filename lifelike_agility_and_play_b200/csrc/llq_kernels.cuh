@@ -17,9 +17,19 @@
 
 namespace llq {
 
-constexpr int kObsDim = 207, kObsDimEpmc = 916, kObsDimSepmc = 965, kPropDim = 33, kActDim = 12, kStateDim = 37, kAuxDim = 18;
-template <int ENV> struct ObsW { static constexpr int value = (ENV == 1 || ENV == 3) ? kObsDimEpmc : (ENV == 2 ? kObsDimSepmc : kObsDim); };
-constexpr int kMaxBoxes = 36, kMaxCand = 12;   // ENV 3 = EPMC corridor (elements 1-3): static boxes per env, contact candidates per step
+constexpr int kObsDim = LLQ_OBS_DIM, kObsDimEpmc = LLQ_OBS_DIM_EPMC, kObsDimSepmc = LLQ_OBS_DIM_SEPMC, kPropDim = LLQ_PROP_DIM, kActDim = LLQ_ACTION_DIM;
+// Kernel instances: the template argument ENV of llq_step16_kernel and pmc_reset_kernel (a handle runs one, llq_cuda.cu).
+// kEpmc is the flat EPMC arena (element 0), kCorridor the EPMC corridor (elements 1-3).
+enum : int { kPmc = 0, kEpmc = 1, kSepmc = 2, kCorridor = 3 };
+__host__ __device__ constexpr bool epmc_like(int env) { return env == kEpmc || env == kCorridor; }
+__host__ __device__ constexpr int obs_width(int env) { return epmc_like(env) ? kObsDimEpmc : (env == kSepmc ? kObsDimSepmc : kObsDim); }
+constexpr int kMaxBoxes = LLQ_MAX_BOXES, kBoxW = 6, kMaxCand = 12;   // EPMC corridor: static boxes per env, floats per box, contact candidates per step
+// Robot state row (LLQ_F_STATE, LLQ_F_KIN_STATE, ModelConst::init_state): base position 3 | orientation xyzw 4 (pybullet inertial frame)
+// | linear velocity 3 | angular velocity 3 | joint positions 12 | joint velocities 12.  EnvArrays::st: the same rows without the position,
+// which EnvArrays::pos keeps in fp64.
+constexpr int kStatePos = 0, kStateQuat = 3, kStateLin = 7, kStateAng = 10, kStateQ = 13, kStateQd = 25;
+constexpr int kStQuat = kStateQuat - 3, kStLin = kStateLin - 3, kStAng = kStateAng - 3, kStQ = kStateQ - 3, kStQd = kStateQd - 3, kStRows = LLQ_STATE_DIM - 3;
+static_assert(kStateQuat == kStatePos + 3 && kStateQd + 12 == LLQ_STATE_DIM, "st = the state row minus the position");
 
 // Staging row: kNewObs floats per env in shared memory.  The step tail and the reset kernel fill it, emit_obs_rows turns it into the
 // observation row.  Shared slots first, then the EPMC names, then the SEPMC names of the same offsets.
@@ -65,7 +75,7 @@ struct BaseConst { float qI[4]; float m; float h[3]; float I[6]; int nd; DampIte
 struct alignas(16) ModelConst {
   BaseConst base; LegConst leg[4];
   float push_R[9]; float push_c[3];   // FR hip link: inertial-frame rotation (link <- inertial) and CoM, for applyExternalForce(LINK_FRAME) (PR:73-77)
-  float init_state[37]; float pad_[3]; // EPMC episode start state (LR:115-117, utils/constants.py:103-116)
+  float init_state[LLQ_STATE_DIM]; float pad_[3]; // EPMC episode start state (LR:115-117, utils/constants.py:103-116)
   // detection proxies for the PMC hurdle plate: wheel (knee) centre in the thigh frame + radius, hip radius, body-box corners (base coords)
   float wheel_off[4][3]; float wheel_r[4]; float hip_r[4]; float corner[8][3];
   float handle[2][4];                  // SEPMC: front / hind handle centre (base coords) + radius (LR:150-156)
@@ -93,7 +103,7 @@ struct StepParams {
 
 struct EnvArrays {      // SoA device arrays, N envs
   double* pos;          // [3][N]
-  float* st;            // [34][N]: quat4 lin3 ang3 q12 qd12
+  float* st;            // [kStRows][N]: the state row without the position, rows kSt*
   double* time;         // [N]
   int* clip;            // [N]
   float* reward_sum;    // [N]
@@ -101,7 +111,7 @@ struct EnvArrays {      // SoA device arrays, N envs
   long long* episode;   // [N]
   float* warm;          // [LLQ_MAX_SPHERES][N]
   float* obs;           // [N][obs width] (history carry)
-  float* kin;           // [37][N]
+  float* kin;           // [LLQ_STATE_DIM][N]: kinematic (mocap) state row, slots kState*
   float* foot_pos;      // [12][N]
   float* done_reward;   // [N] reward_sum at termination
   unsigned char* done;  // [N]
@@ -109,7 +119,7 @@ struct EnvArrays {      // SoA device arrays, N envs
   unsigned long long* counters;  // [8]
   double* aux;          // [LLQ_AUX_DIM][N] EPMC / SEPMC bookkeeping, slots LLQ_AUX_* (include/llq.h)
   int* ob_id;           // [N] active hurdle plate
-  float* boxes;         // [N][36][6] EPMC corridor: centre xyz, half extents xyz (walls first)
+  float* boxes;         // [N][kMaxBoxes][kBoxW] EPMC corridor: centre xyz, half extents xyz (walls first)
   int* nbox;            // [N]
 };
 
@@ -197,13 +207,13 @@ LLQ_DI void write_robot(const EnvArrays& E, int N, int env, int k, const float (
                         double pz, Q4 qb, V3 lin, V3 ang, double time) {
   float* sw = E.st;
 #pragma unroll
-  for (int t = 0; t < 3; t++) { sw[(10 + 3 * k + t) * N + env] = q[t]; sw[(22 + 3 * k + t) * N + env] = qd[t]; }
+  for (int t = 0; t < 3; t++) { sw[(kStQ + 3 * k + t) * N + env] = q[t]; sw[(kStQd + 3 * k + t) * N + env] = qd[t]; }
   E.foot_pos[(3 * k) * N + env] = foot.x; E.foot_pos[(3 * k + 1) * N + env] = foot.y; E.foot_pos[(3 * k + 2) * N + env] = foot.z;
   if (k == 0) {
     E.pos[env] = px; E.pos[N + env] = py; E.pos[2 * N + env] = pz;
     const float b[10] = {qb.x, qb.y, qb.z, qb.w, lin.x, lin.y, lin.z, ang.x, ang.y, ang.z};
 #pragma unroll
-    for (int t = 0; t < 10; t++) sw[t * N + env] = b[t];
+    for (int t = 0; t < 10; t++) sw[(kStQuat + t) * N + env] = b[t];
     E.time[env] = time;
   }
 }
@@ -427,7 +437,7 @@ LLQ_DI void sepmc_pair_tail(const ModelConst& M, const LegConst& L, int k, int r
 LLQ_DI unsigned long long box_mask(const float* boxes, int nb, int k, float px, float py, float pz, float margin, bool zsel) {
   unsigned long long m = 0ull;
   for (int j = k; j < nb; j += 4) {
-    const float* b = boxes + 6 * j;
+    const float* b = boxes + kBoxW * j;
     const bool hit = zsel ? fabsf(b[2] - pz) <= b[5] : (fabsf(b[0] - px) <= b[3] + margin && fabsf(b[1] - py) <= b[4] + margin);
     if (hit) m |= 1ull << j;
   }
@@ -446,7 +456,7 @@ LLQ_DI float ray_boxlist(V3 o, V3 d, const float* boxes, unsigned long long mask
   while (mask) {
     const int j = __ffsll((long long)mask) - 1;
     mask &= mask - 1;
-    const float* b = boxes + 6 * j;
+    const float* b = boxes + kBoxW * j;
     const V3 lo = V3{b[0] - b[3], b[1] - b[4], b[2] - b[5]}, hi = V3{b[0] + b[3], b[1] + b[4], b[2] + b[5]};
     if (lo.x > x1 || hi.x < x0 || lo.y > y1 || hi.y < y0 || lo.z > z1 || hi.z < z0) continue;
     best = ray_box1(o, d, lo, hi, best);
@@ -460,7 +470,7 @@ LLQ_DI float down_ray_top(float x, float y, const float* boxes, unsigned long lo
   while (mask) {
     const int j = __ffsll((long long)mask) - 1;
     mask &= mask - 1;
-    const float* b = boxes + 6 * j;
+    const float* b = boxes + kBoxW * j;
     const bool out = x < b[0] - b[3] || x > b[0] + b[3] || y < b[1] - b[4] || y > b[1] + b[4];
     if (!out) top = fmaxf(top, b[2] + b[5]);
   }
@@ -479,7 +489,7 @@ struct TerrainRng {
 };
 LLQ_DI void put_box(float* boxes, int& nb, bool wr, double cx, double cy, double cz, double lx, double ly, double lz) {
   if (nb < kMaxBoxes && wr) {
-    float* b = boxes + 6 * nb;
+    float* b = boxes + kBoxW * nb;
     b[0] = (float)cx; b[1] = (float)cy; b[2] = (float)cz; b[3] = (float)(lx / 2); b[4] = (float)(ly / 2); b[5] = (float)(lz / 2);
   }
   if (nb < kMaxBoxes) nb++;
@@ -628,7 +638,7 @@ LLQ_DI void front_ray(const float* sn, int t, V3& from, V3& d) {
 template <int ENV, int EPW = 8>   // EPW = envs per warp (8 with 4 lanes per env, 2 with 16)
 LLQ_DI void emit_obs_rows(float* obs, float* obs2, long long obs2_ld, const float* snew_warp, const float* hist_warp, int env0, int n_envs,
                           int mode, unsigned row_mask, const float* boxes_all = nullptr) {
-  constexpr int OW = ObsW<ENV>::value;
+  constexpr int OW = obs_width(ENV);
   const int lane = threadIdx.x & 31;
 #pragma unroll 4
   for (int base = 0; base < EPW * OW; base += 32) {
@@ -646,12 +656,12 @@ LLQ_DI void emit_obs_rows(float* obs, float* obs2, long long obs2_ld, const floa
         int a = j - kOPropA;
         if (mode == 1) v = 0.f;
         else v = a < kHistAct ? hs[kHistProp + a] : sn[kSAct + a - kHistAct];
-      } else if (ENV == 0) {
+      } else if (ENV == kPmc) {
         v = sn[kSFuture + (j - kOFuture)];
-      } else if (ENV == 3) {
+      } else if (ENV == kCorridor) {
         // EPMC corridor perception against the ground slab and the env's candidate boxes (PGE:374-447)
         const V3 pos = ld3(sn + kSPos);
-        const float* bxs = boxes_all + (size_t)(env0 + e) * (6 * kMaxBoxes);
+        const float* bxs = boxes_all + (size_t)(env0 + e) * (kBoxW * kMaxBoxes);
         if (j < kOLidar) {
           const float2 g = grid_point(sn, j - kOGrid);
           v = fmaxf(down_ray_top(g.x, g.y, bxs, staged_mask(sn, kSMaskGrid)), 0.f);   // hit z of the down ray (0 when it misses everything)
@@ -667,7 +677,7 @@ LLQ_DI void emit_obs_rows(float* obs, float* obs2, long long obs2_ld, const floa
         } else {
           v = sn[kSTarget + (j - kOTail)];
         }
-      } else if (ENV == 2) {
+      } else if (ENV == kSepmc) {
         // SEPMC perception against ground slab, walls and flag (CTG:598-638, PGE:22-54)
         const V3 pos = ld3(sn + kSPos);
         const float fx = sn[kSFlag], fy = sn[kSFlag + 1];
@@ -721,7 +731,7 @@ LLQ_DI void emit_obs_rows(float* obs, float* obs2, long long obs2_ld, const floa
 // Asynchronous (cp.async) prefetch issued at kernel start; consumed after the ten sub-steps, so DRAM latency is hidden.
 template <int ENV, int EPW = 8>
 LLQ_DI void prefetch_history(const float* obs, float* hist_warp, int env0, int n_envs) {
-  constexpr int OW = ObsW<ENV>::value;
+  constexpr int OW = obs_width(ENV);
   const int lane = threadIdx.x & 31;
   for (int idx = lane; idx < EPW * kHist; idx += 32) {
     int e = idx / kHist, t = idx - e * kHist;
@@ -763,10 +773,10 @@ LLQ_DI StartPose start_pose(const ModelConst& M, int k, double yaw_deg) {
   double sn, cs;
   sincos(0.5 * yaw_deg * (3.14159265358979323846 / 180.0), &sn, &cs);
   const float* I0 = M.init_state;
-  s.qn = qmul(qnormalize(Q4{I0[3], I0[4], I0[5], I0[6]}), Q4{0.f, 0.f, (float)sn, (float)cs});
+  s.qn = qmul(qnormalize(Q4{I0[kStateQuat], I0[kStateQuat + 1], I0[kStateQuat + 2], I0[kStateQuat + 3]}), Q4{0.f, 0.f, (float)sn, (float)cs});
 #pragma unroll
-  for (int i = 0; i < 3; i++) { s.q[i] = I0[13 + 3 * k + i]; s.qd[i] = I0[25 + 3 * k + i]; }
-  s.lin = V3{I0[7], I0[8], I0[9]}; s.ang = V3{I0[10], I0[11], I0[12]};
+  for (int i = 0; i < 3; i++) { s.q[i] = I0[kStateQ + 3 * k + i]; s.qd[i] = I0[kStateQd + 3 * k + i]; }
+  s.lin = ld3(I0 + kStateLin); s.ang = ld3(I0 + kStateAng);
   const Q4 qI = Q4{M.base.qI[0], M.base.qI[1], M.base.qI[2], M.base.qI[3]};
   s.qp = qmul(qnormalize(s.qn), qconj(qI));
   return s;
@@ -833,12 +843,12 @@ __global__ void __launch_bounds__(kResetBlock) pmc_reset_kernel(EnvArrays E, Moc
   bool doit = valid;
   if (RP.mode == 3) doit = false;
   else if (RP.mode == 0) doit = doit && E.done[env] != 0;
-  else if (RP.mask) doit = doit && (RP.mask[env] != 0 || (ENV == 2 && RP.mask[env ^ 1] != 0));   // SEPMC: a pair resets as a whole
+  else if (RP.mask) doit = doit && (RP.mask[env] != 0 || (ENV == kSepmc && RP.mask[env ^ 1] != 0));   // SEPMC: a pair resets as a whole
   const unsigned wm = __ballot_sync(FULL, doit);
   if (wm == 0) return;                                   // warp-uniform: nothing to reset in these 8 envs
   const LegConst& L = M.leg[k];
 
-  if (ENV == 2) {
+  if (ENV == kSepmc) {
     // ---------------- SEPMC reset (CTG:261-304, 204-230); draws keyed by the pair: stream 1 = [fix_spd, with_flag, friction, x0 |
     // y0, x1, y1, yaw0 | yaw1, flag x, flag y]
     const int robot = env & 1;
@@ -880,7 +890,7 @@ __global__ void __launch_bounds__(kResetBlock) pmc_reset_kernel(EnvArrays E, Moc
         A[LLQ_AUX_FLAG_DRAWS * N + env] = PS.flag_draws; A[LLQ_AUX_YAW_ACCUM_DEG * N + env] = yaw_b; A[LLQ_AUX_FLAG_TOUCH * N + env] = touch_own ? 1.0 : 0.0;
       }
     }
-  } else if (ENV == 1 || ENV == 3) {
+  } else if (epmc_like(ENV)) {
     // ---------------- EPMC reset (PGE:196-249)
     long long ep = E.episode[env];
     const long long gid = RP.gid0 + env;
@@ -895,7 +905,7 @@ __global__ void __launch_bounds__(kResetBlock) pmc_reset_kernel(EnvArrays E, Moc
     const float target_spd = (float)E.aux[LLQ_AUX_TARGET_SPD * N + env];            // persists across episodes (PGE:170-172)
     double tgx0 = 8.0;
     int nb0 = 0;
-    if (ENV == 3) nb0 = generate_corridor(P, RP.seed, gid, ep, E.boxes + (size_t)env * (6 * kMaxBoxes), doit && k == 0, tgx0);   // PGE:216-219
+    if (ENV == kCorridor) nb0 = generate_corridor(P, RP.seed, gid, ep, E.boxes + (size_t)env * (kBoxW * kMaxBoxes), doit && k == 0, tgx0);   // PGE:216-219
     // the pose after the corridor: generated before it, it is live across generate_corridor (registers).  qn is a local copy and the
     // foot below keeps the expression with its own qp: read through S or from S.qp, nvcc contracts the quaternion arithmetic differently
     // and element 0's foot positions change in the last bit.
@@ -908,9 +918,9 @@ __global__ void __launch_bounds__(kResetBlock) pmc_reset_kernel(EnvArrays E, Moc
       stage_pose(snew, Rq, tmul(Rq, S.ang), tmul(Rq, S.lin), V3{0.f, 0.f, 0.5f});
       stage_target(snew, Rq, 0.0, 0.0, 0.5, tgx0, 0.0, target_spd);                 // element 0: target (8, 0, 0) (BSE:247-248)
     }
-    if (ENV == 3) {
+    if (ENV == kCorridor) {
       __syncwarp();                                                 // lane 0's boxes are visible to the env's other lanes
-      stage_corridor_masks(snew, E.boxes + (size_t)env * (6 * kMaxBoxes), doit ? nb0 : E.nbox[env], k, 0.f, 0.f, 0.5f, atan2f(Rq.a10, Rq.a00));
+      stage_corridor_masks(snew, E.boxes + (size_t)env * (kBoxW * kMaxBoxes), doit ? nb0 : E.nbox[env], k, 0.f, 0.f, 0.5f, atan2f(Rq.a10, Rq.a00));
     }
     if (doit) {
       const Q4 qI = Q4{M.base.qI[0], M.base.qI[1], M.base.qI[2], M.base.qI[3]};
@@ -922,7 +932,7 @@ __global__ void __launch_bounds__(kResetBlock) pmc_reset_kernel(EnvArrays E, Moc
         A[LLQ_AUX_COUNTER * N + env] = 0; A[LLQ_AUX_CMD_FREQ * N + env] = cmd_freq; A[LLQ_AUX_TARGET_X * N + env] = tgx0;
         A[LLQ_AUX_TARGET_Y * N + env] = 0.0; A[LLQ_AUX_LAST_POS_DIFF_LEN * N + env] = fabs(tgx0); A[LLQ_AUX_TOTAL_SPD * N + env] = 0.0;
         A[LLQ_AUX_INIT_POS_DIFF_LEN * N + env] = fabs(tgx0);                                  // init_pos_diff_len (PGE:192-195)
-        if (ENV == 3) E.nbox[env] = nb0;
+        if (ENV == kCorridor) E.nbox[env] = nb0;
         A[LLQ_AUX_MAX_SPD * N + env] = 0.0; A[LLQ_AUX_PUSH_COUNT * N + env] = P.push_start_count; A[LLQ_AUX_PUSH_F * N + env] = pf[0];
         A[(LLQ_AUX_PUSH_F + 1) * N + env] = pf[1]; A[(LLQ_AUX_PUSH_F + 2) * N + env] = pf[2];
         A[LLQ_AUX_FOOT_FRICTION * N + env] = foot_mu; A[LLQ_AUX_PUSH_DRAWS * N + env] = push_draws; A[LLQ_AUX_CMD_DRAWS * N + env] = 0;
@@ -970,12 +980,12 @@ __global__ void __launch_bounds__(kResetBlock) pmc_reset_kernel(EnvArrays E, Moc
       write_robot(E, N, env, k, q, qd, fd, kb.px, kb.py, kb.pz, kb.q, kb.lin, kb.ang, t0);
       write_reset(E, N, env, k, ep);
 #pragma unroll
-      for (int i = 0; i < 3; i++) { E.kin[(13 + 3 * k + i) * N + env] = q[i]; E.kin[(25 + 3 * k + i) * N + env] = qd[i]; }
+      for (int i = 0; i < 3; i++) { E.kin[(kStateQ + 3 * k + i) * N + env] = q[i]; E.kin[(kStateQd + 3 * k + i) * N + env] = qd[i]; }
       if (k == 0) {
         const float b[10] = {kb.q.x, kb.q.y, kb.q.z, kb.q.w, kb.lin.x, kb.lin.y, kb.lin.z, kb.ang.x, kb.ang.y, kb.ang.z};
-        E.kin[env] = (float)kb.px; E.kin[N + env] = (float)kb.py; E.kin[2 * N + env] = (float)kb.pz;
+        E.kin[kStatePos * N + env] = (float)kb.px; E.kin[(kStatePos + 1) * N + env] = (float)kb.py; E.kin[(kStatePos + 2) * N + env] = (float)kb.pz;
 #pragma unroll
-        for (int i = 0; i < 10; i++) E.kin[(3 + i) * N + env] = b[i];
+        for (int i = 0; i < 10; i++) E.kin[(kStateQuat + i) * N + env] = b[i];
         E.clip[env] = clip;
         E.ob_id[env] = 0;                                            // PLE:179
       }

@@ -648,8 +648,8 @@ LLQ_DI void step_tail(const EnvArrays& E, const MocapDev& mc, const StepParams& 
   float q[3], qd[3];
 #pragma unroll
   for (int t = 0; t < 3; t++) { q[t] = T.q[3 * k + t]; qd[t] = T.qd[3 * k + t]; }
-  const int clip = ENV == 0 ? E.clip[env] : 0;
-  const long long epi = ENV != 0 ? E.episode[ENV == 2 ? env & ~1 : env] - 1 : 0;   // SEPMC: the pair's id is robot 0's
+  const int clip = ENV == kPmc ? E.clip[env] : 0;
+  const long long epi = ENV != kPmc ? E.episode[ENV == kSepmc ? env & ~1 : env] - 1 : 0;   // SEPMC: the pair's id is robot 0's
   const int robot = env & 1;
   const long long pair_gid = gid0 + (env & ~1);
   bool done = false;
@@ -659,7 +659,7 @@ LLQ_DI void step_tail(const EnvArrays& E, const MocapDev& mc, const StepParams& 
   const Q4 qI = Q4{M.base.qI[0], M.base.qI[1], M.base.qI[2], M.base.qI[3]};
   const Q4 qb = qmul(qp, qI);                          // back to the pybullet (inertial-frame) convention
   PairState PS = {0, 0, 1, 0, 0.0, 0.0};
-  if (ENV == 0) {
+  if (ENV == kPmc) {
     float* snew = s_new + el * kNewObs;
     ObsCtx oc = build_obs_new(mc, P, M, k, clip, frame_id, frame_frac, px, py, pz, qb, vw, ww, q, qd, snew);
 #pragma unroll
@@ -701,21 +701,23 @@ LLQ_DI void step_tail(const EnvArrays& E, const MocapDev& mc, const StepParams& 
     if (wr) {
       write_robot(E, N, env, k, q, qd, fd, px, py, pz, qb, vw, ww, time);
 #pragma unroll
-      for (int t = 0; t < 3; t++) { E.kin[(13 + 3 * k + t) * N + env] = oc.kq[t]; E.kin[(25 + 3 * k + t) * N + env] = oc.kqd[t]; }
+      for (int t = 0; t < 3; t++) { E.kin[(kStateQ + 3 * k + t) * N + env] = oc.kq[t]; E.kin[(kStateQd + 3 * k + t) * N + env] = oc.kqd[t]; }
       if (k == 0) {
         if (P.has_ob) E.ob_id[env] = ob_id;
         const float rs = write_step(E, env, rew, done);
-        E.kin[env] = (float)oc.kb.px; E.kin[N + env] = (float)oc.kb.py; E.kin[2 * N + env] = (float)oc.kb.pz;
-        E.kin[3 * N + env] = oc.kb.q.x; E.kin[4 * N + env] = oc.kb.q.y; E.kin[5 * N + env] = oc.kb.q.z; E.kin[6 * N + env] = oc.kb.q.w;
-        E.kin[7 * N + env] = oc.kb.lin.x; E.kin[8 * N + env] = oc.kb.lin.y; E.kin[9 * N + env] = oc.kb.lin.z;
-        E.kin[10 * N + env] = oc.kb.ang.x; E.kin[11 * N + env] = oc.kb.ang.y; E.kin[12 * N + env] = oc.kb.ang.z;
+        E.kin[kStatePos * N + env] = (float)oc.kb.px; E.kin[(kStatePos + 1) * N + env] = (float)oc.kb.py;
+        E.kin[(kStatePos + 2) * N + env] = (float)oc.kb.pz;
+        E.kin[kStateQuat * N + env] = oc.kb.q.x; E.kin[(kStateQuat + 1) * N + env] = oc.kb.q.y; E.kin[(kStateQuat + 2) * N + env] = oc.kb.q.z;
+        E.kin[(kStateQuat + 3) * N + env] = oc.kb.q.w;
+        E.kin[kStateLin * N + env] = oc.kb.lin.x; E.kin[(kStateLin + 1) * N + env] = oc.kb.lin.y; E.kin[(kStateLin + 2) * N + env] = oc.kb.lin.z;
+        E.kin[kStateAng * N + env] = oc.kb.ang.x; E.kin[(kStateAng + 1) * N + env] = oc.kb.ang.y; E.kin[(kStateAng + 2) * N + env] = oc.kb.ang.z;
         if (done) {
           E.done_reward[env] = rs;
           atomicMax(&winner[clip], env);       // highest finished env index owns the clip's slot this step (PLE:236)
         }
       }
     }
-  } else if (ENV == 2) {
+  } else if (ENV == kSepmc) {
     // ---------------- SEPMC tail (CTG:378-424, 458-470, 495-596, 640-652)
     const double* A = E.aux;
     int counter = (int)A[LLQ_AUX_COUNTER * N + env];
@@ -768,14 +770,14 @@ LLQ_DI void step_tail(const EnvArrays& E, const MocapDev& mc, const StepParams& 
     double target_angle = A[LLQ_AUX_TARGET_ANGLE * N + env], last_len = A[LLQ_AUX_LAST_POS_DIFF_LEN * N + env];
     double total_spd = A[LLQ_AUX_TOTAL_SPD * N + env], max_spd = A[LLQ_AUX_MAX_SPD * N + env];
     float target_spd = (float)A[LLQ_AUX_TARGET_SPD * N + env];
-    const double init_len = ENV == 3 ? A[LLQ_AUX_INIT_POS_DIFF_LEN * N + env] : 1.0;
+    const double init_len = ENV == kCorridor ? A[LLQ_AUX_INIT_POS_DIFF_LEN * N + env] : 1.0;
     {
       // the command of this step was drawn from the pose at the START of the step (PGE:302-317): recover it from the stored state
       const double sx0 = E.pos[env], sy0 = E.pos[N + env];
       if (counter % cmd_freq == 0) {
         double uu[4];
         stream_uniforms(seed, gid0 + env, epi, 3, (unsigned)cmd_draws++, uu);
-        if (ENV == 1) {
+        if (ENV == kEpmc) {
           target_angle = 2.0 * 3.14159265358979323846 * uu[0];
           double sn, cs;
           sincos(target_angle, &sn, &cs);
@@ -784,7 +786,7 @@ LLQ_DI void step_tail(const EnvArrays& E, const MocapDev& mc, const StepParams& 
         }
         target_spd = (float)((double)P.ts_lo + uu[1] * ((double)P.ts_hi - (double)P.ts_lo));
       }
-      if (ENV == 3) target_angle = atan2(tgy - sy0, tgx - sx0);            // PGE:318-323 (plotting only)
+      if (ENV == kCorridor) target_angle = atan2(tgy - sy0, tgx - sx0);    // PGE:318-323 (plotting only)
     }
     __syncwarp();                                        // the pose above is read before lane 0 overwrites it below
     float* snew = s_new + el * kNewObs;
@@ -810,13 +812,13 @@ LLQ_DI void step_tail(const EnvArrays& E, const MocapDev& mc, const StepParams& 
     float sy_, cy_;
     llq_sincosf(yaw, &sy_, &cy_);
     float rew = expf(-fabsf(spd - target_spd)) * expf((cy_ * ux + sy_ * uy - 1.0f) * 5.0f) / (float)P.max_steps;
-    if (ENV == 3) {                                                    // _compute_avg_spd_reward (PGE:504-539)
+    if (ENV == kCorridor) {                                            // _compute_avg_spd_reward (PGE:504-539)
       const float reward_rot = expf((cy_ * ux + sy_ * uy - 1.0f) * 5.0f);
       const float reward_dist = (float)((plen - last_len) / init_len);
       last_len = plen;
       rew = reward_rot / (float)P.max_steps * 0.1f * 2.0f - reward_dist * 0.1f;
       if (reach) rew += expf(-fabsf((float)(total_spd / (double)counter) - target_spd));
-      stage_corridor_masks(snew, E.boxes + (size_t)env * (6 * kMaxBoxes), E.nbox[env], k, (float)px, (float)py, (float)pz, yaw);
+      stage_corridor_masks(snew, E.boxes + (size_t)env * (kBoxW * kMaxBoxes), E.nbox[env], k, (float)px, (float)py, (float)pz, yaw);
     }
     if (bad || !isfinite(rew)) { rew = 0.f; bad = true; }
     done = fall || timeup || reach || bad;
@@ -839,14 +841,14 @@ LLQ_DI void step_tail(const EnvArrays& E, const MocapDev& mc, const StepParams& 
   // record mode (llq_set_option "record"): the trajectory columns action 12 | reward | done behind the observation of the slab row;
   // record == 2: into the slab row before the one that receives the observation (parallel/rollout.py)
   if (record && obs2 && wr) {
-    float* row = obs2 + (size_t)env * obs2_ld + ObsW<ENV>::value - (record == 2 ? (long long)N * obs2_ld : 0ll);
+    float* row = obs2 + (size_t)env * obs2_ld + obs_width(ENV) - (record == 2 ? (long long)N * obs2_ld : 0ll);
 #pragma unroll
     for (int t = 0; t < 3; t++) row[3 * k + t] = act_src[3 * k + t];
     if (k == 0) { row[12] = rew_out; row[13] = done ? 1.f : 0.f; }
   }
   {
     const unsigned dm = __ballot_sync(FULL, valid && k == 0 && done);       // episodes finished: one atomic per warp
-    if ((threadIdx.x & 31) == 0 && dm) atomicAdd(&E.counters[1], (unsigned long long)__popc(dm));
+    if ((threadIdx.x & 31) == 0 && dm) atomicAdd(&E.counters[LLQ_CNT_EPISODES], (unsigned long long)__popc(dm));
   }
   // (the observation rows are emitted by ALL warps of the CTA after a barrier: kernel epilogue)
 }
@@ -904,14 +906,14 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
   // ---- load state (base entries replicated on the 16 lanes, joint entries on the 4 lanes of the leg)
   double px = E.pos[env], py = E.pos[N + env], pz = E.pos[2 * N + env];
   const float* st = E.st;
-  Q4 qb = Q4{st[env], st[N + env], st[2 * N + env], st[3 * N + env]};
-  V3 vw = V3{st[4 * N + env], st[5 * N + env], st[6 * N + env]};
-  V3 ww = V3{st[7 * N + env], st[8 * N + env], st[9 * N + env]};
+  Q4 qb = Q4{st[kStQuat * N + env], st[(kStQuat + 1) * N + env], st[(kStQuat + 2) * N + env], st[(kStQuat + 3) * N + env]};
+  V3 vw = V3{st[kStLin * N + env], st[(kStLin + 1) * N + env], st[(kStLin + 2) * N + env]};
+  V3 ww = V3{st[kStAng * N + env], st[(kStAng + 1) * N + env], st[(kStAng + 2) * N + env]};
   float q[3], qd[3];
 #pragma unroll
   for (int t = 0; t < 3; t++) {
-    q[t] = st[(10 + 3 * k + t) * N + env];
-    qd[t] = st[(22 + 3 * k + t) * N + env];
+    q[t] = st[(kStQ + 3 * k + t) * N + env];
+    qd[t] = st[(kStQd + 3 * k + t) * N + env];
   }
   if (i < 3) {                                               // joint (k, i): action and clipped target stay in shared memory
     const float a = actions[(size_t)env * kActDim + 3 * k + i];
@@ -923,10 +925,10 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
   warm[0] = l16 < nsph ? E.warm[(size_t)l16 * N + env] : 0.f;
   warm[1] = 16 + l16 < nsph ? E.warm[(size_t)(16 + l16) * N + env] : 0.f;
   double time = E.time[env];
-  const int clip = ENV == 0 ? E.clip[env] : 0;
+  const int clip = ENV == kPmc ? E.clip[env] : 0;
   int frame_id = 0; double frame_frac = 0.0;
   int ob_id = 0; bool ob_hit = false;
-  if (ENV == 0 && P.has_ob) ob_id = E.ob_id[env];
+  if (ENV == kPmc && P.has_ob) ob_id = E.ob_id[env];
   // ---- EPMC / SEPMC bookkeeping used inside the sub-steps (the rest is read in the tail)
   int push_count = 0, push_draws = 0;
   float pf[3] = {0.f, 0.f, 0.f}, mu_env = P.mu;
@@ -935,20 +937,20 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
   bool touch_own = false, tag = false;
   const int robot = env & 1;
   const long long pair_gid = gid0 + (env & ~1);
-  if (ENV != 0) {
+  if (ENV != kPmc) {
     const double* A = E.aux;
     push_count = (int)A[LLQ_AUX_PUSH_COUNT * N + env];
     pf[0] = (float)A[LLQ_AUX_PUSH_F * N + env]; pf[1] = (float)A[(LLQ_AUX_PUSH_F + 1) * N + env]; pf[2] = (float)A[(LLQ_AUX_PUSH_F + 2) * N + env];
     mu_env = P.mu_ground * (float)A[LLQ_AUX_FOOT_FRICTION * N + env]; push_draws = (int)A[LLQ_AUX_PUSH_DRAWS * N + env];
-    epi = E.episode[ENV == 2 ? env & ~1 : env] - 1;       // streams of the running episode (the reset advanced the counter); SEPMC: robot 0's
-    if (ENV == 2) { PS.flag_x = A[LLQ_AUX_FLAG_X * N + env]; PS.flag_y = A[LLQ_AUX_FLAG_Y * N + env]; }
+    epi = E.episode[ENV == kSepmc ? env & ~1 : env] - 1;       // streams of the running episode (the reset advanced the counter); SEPMC: robot 0's
+    if (ENV == kSepmc) { PS.flag_x = A[LLQ_AUX_FLAG_X * N + env]; PS.flag_y = A[LLQ_AUX_FLAG_Y * N + env]; }
   }
   // ---- EPMC corridor: the boxes the robot can reach during this step -> shared memory (<= kMaxCand per env)
   int n_cand = 0;
   float* s_cand = nullptr;
-  if (ENV == 3) {
+  if (ENV == kCorridor) {
     s_cand = s_new[el];                            // the staging row is free until the tail: 8 x 6 floats
-    const float* bxs = E.boxes + (size_t)env * (6 * kMaxBoxes);
+    const float* bxs = E.boxes + (size_t)env * (kBoxW * kMaxBoxes);
     // reach of the robot's spheres from the base reference point: hip offset 0.195 + leg 0.48 in x, 0.15 + 0.05 in y, plus the
     // travel during the step (<= 0.06 m at 3 m/s) -> 0.8 m per axis (0.6 missed hind feet stretched backwards over a hurdle)
     unsigned long long m = box_mask(bxs, E.nbox[env], k, (float)px, (float)py, (float)pz, 0.8f, false);
@@ -958,7 +960,7 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
       m &= m - 1;
       if ((c & 3) == k && i == 0) {
 #pragma unroll
-        for (int t = 0; t < 6; t++) s_cand[6 * c + t] = bxs[6 * j + t];
+        for (int t = 0; t < kBoxW; t++) s_cand[kBoxW * c + t] = bxs[kBoxW * j + t];
       }
       c++;
     }
@@ -970,7 +972,7 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
   Q4 qp = qmul(qnormalize(qb), qconj(qI));
   unsigned n_contact_rows = 0, n_limit_rows = 0, n_overflow = 0;
   bool bad = false;
-  const float mu_foot = ENV != 0 ? mu_env : P.mu;
+  const float mu_foot = ENV != kPmc ? mu_env : P.mu;
 
   T16_DECL;
   for (int sub = 0; sub < P.substeps; sub++) {
@@ -978,7 +980,7 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
     const float dt = P.dt;
     // ---------------- push randomiser (PR:56-87): counters in sub-steps, force lasts one sub-step
     bool push_on = false;
-    if (ENV == 2 && P.push_enabled) {
+    if (ENV == kSepmc && P.push_enabled) {
       push_count += 1;
       if (push_count > 0) {
         if (push_count % P.push_interval == 0) { push_draws += 1; push_count = 0; }
@@ -990,7 +992,7 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
         }
       }
     }
-    if ((ENV == 1 || ENV == 3) && P.push_enabled) {
+    if (epmc_like(ENV) && P.push_enabled) {
       push_count += 1;
       if (push_count > 0) {
         if (push_count % P.push_interval == 0) { epmc_randomize_push(P, seed, gid0 + env, epi, push_draws, pf); push_count = 0; }
@@ -1048,7 +1050,7 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
     SV f = bias_wrench(bm_, hc, Ic, nd, dp, v.a, v.l, P.kl, P.ka, cy, sy, cx, sx, po);
     f.a = f.a + mul(Ic, ab.a) + cross(hc, ab.l);
     f.l = f.l + bm_ * ab.l + cross(ab.a, hc);
-    if (ENV != 0 && push_on && l16 == 0) {
+    if (ENV != kPmc && push_on && l16 == 0) {
       // applyExternalForce(link 0 = FR hip, LINK_FRAME): force given in the hip's inertial frame, applied at its CoM (PR:73-77)
       const V3 fl = V3{M.push_R[0] * pf[0] + M.push_R[1] * pf[1] + M.push_R[2] * pf[2], M.push_R[3] * pf[0] + M.push_R[4] * pf[1] + M.push_R[5] * pf[2],
                        M.push_R[6] * pf[0] + M.push_R[7] * pf[1] + M.push_R[8] * pf[2]};
@@ -1123,7 +1125,7 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
     __syncwarp();
     const M3 R = qmat(qp);                            // world <- B' (recomputed: cheaper than keeping nine registers alive)
     // ---------------- PMC hurdle plate: getContactPoints (PLE:343) reports the manifolds built on the last sub-step's pre-step poses
-    if (ENV == 0 && P.has_ob && sub == P.substeps - 1) {
+    if (ENV == kPmc && P.has_ob && sub == P.substeps - 1) {
       const int o0 = mc.ob_off[clip], n_ob = mc.ob_off[clip + 1] - o0;
       if (n_ob > 0) {
         const LegFrames lf = leg_frames(linktab, k);
@@ -1142,7 +1144,7 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
       }
     }
     // ---------------- SEPMC: getContactPoints() (CTG:426-456) = manifolds of the last sub-step, built on its pre-step poses
-    if (ENV == 2 && sub == P.substeps - 1) {
+    if (ENV == kSepmc && sub == P.substeps - 1) {
       float* srow = s_new[el];
       const float* prow = s_new[el ^ 1];
       const V3 pw = V3{(float)px, (float)py, (float)pz};
@@ -1207,16 +1209,16 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
         float dist = (float)pz + dot(nb, cb) - sp.r;                // fp32 screen
         const bool statics = rule == 2 || s < 4;                    // legacy rules: only the feet touch walls and boxes
         bool near_ = have && dist < P.breaking + 0.01f;
-        if (ENV == 2 && statics && have) {
+        if (ENV == kSepmc && statics && have) {
           const V3 cw = V3{(float)px, (float)py, (float)pz} + mul(R, cb);
           near_ = near_ || fmaxf(fabsf(cw.x), fabsf(cw.y)) + sp.r > kWallIn - P.breaking - 0.01f;
         }
         unsigned cmask = 0;                              // ENV 3: candidate boxes this sphere can touch (fp32 screen, 3 cm of slack)
-        if (ENV == 3 && statics && have && n_cand > 0) {
+        if (ENV == kCorridor && statics && have && n_cand > 0) {
           const V3 cw = V3{(float)px, (float)py, (float)pz} + mul(R, cb);
           const float reach = sp.r + P.aux_r + P.breaking + 0.03f;
           for (int c = 0; c < n_cand; c++) {
-            const float* bx = s_cand + 6 * c;
+            const float* bx = s_cand + kBoxW * c;
             const float ex = fabsf(cw.x - bx[0]) - bx[3], ey = fabsf(cw.y - bx[1]) - bx[4], ez = fabsf(cw.z - bx[2]) - bx[5];
             if (fmaxf(ex, fmaxf(ey, ez)) < reach) cmask |= 1u << c;
           }
@@ -1246,10 +1248,10 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
               x += (double)SL.j[0].r[0]; y += (double)SL.j[0].r[1]; z += (double)SL.j[0].r[2];
             }
             dist = (float)(pz + nx * x + ny * y + nz * z - (double)sp.r);
-            if ((ENV == 2 || ENV == 3) && statics) {
+            if ((ENV == kSepmc || ENV == kCorridor) && statics) {
               const double wx = px + (1.0 - 2.0 * (qy * qy + qz * qz)) * x + 2.0 * (qx * qy - qz * qw) * y + 2.0 * (qx * qz + qy * qw) * z;
               const double wy = py + 2.0 * (qx * qy + qz * qw) * x + (1.0 - 2.0 * (qx * qx + qz * qz)) * y + 2.0 * (qy * qz - qx * qw) * z;
-              if (ENV == 2) {
+              if (ENV == kSepmc) {
                 // the arena walls (BSG:863-902) as four more half-spaces; one contact per sphere, the deepest (DESIGN.md 5)
                 const double lim = (double)kWallIn - (double)sp.r;
                 const float d1 = (float)(lim - wx), d2 = (float)(lim + wx), d3 = (float)(lim - wy), d4 = (float)(lim + wy);
@@ -1263,7 +1265,7 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
                 for (unsigned cm = cmask; cm; cm &= cm - 1) {
                   const int c = __ffs((int)cm) - 1;
                   double db; V3 nn;
-                  const float* bx = s_cand + 6 * c;
+                  const float* bx = s_cand + kBoxW * c;
                   sphere_box(wx, wy, wz, (double)sp.r, bx, db, nn);
                   if ((float)db < dist) { dist = (float)db; plane = 5; nworld = nn; }
                   // the element's two auxiliary cylinders (BSE:43-104): along y on the box's x faces, on its top edge (bars: bottom edge);
@@ -1298,7 +1300,7 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
         if (contact) {
           // directions (base coordinates): normal, then btPlaneSpace1's two tangents
           V3 dn = nb, d1_ = neg(V3{R.a10, R.a11, R.a12}), d2_ = V3{R.a00, R.a01, R.a02};   // ground: n = +z, t1 = -y, t2 = +x (world)
-          if (ENV == 2 && plane != 0) {
+          if (ENV == kSepmc && plane != 0) {
             const V3 w0 = V3{R.a00, R.a01, R.a02}, w1 = V3{R.a10, R.a11, R.a12};
             d2_ = nb;                                     // t2 = +z for every wall
             if (plane == 1) { dn = neg(w0); d1_ = neg(w1); }
@@ -1306,7 +1308,7 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
             else if (plane == 3) { dn = neg(w1); d1_ = w0; }
             else { dn = w1; d1_ = neg(w0); }
           }
-          if (ENV == 3 && plane == 5) {                   // general normal: btPlaneSpace1 in world axes, then into base coordinates
+          if (ENV == kCorridor && plane == 5) {           // general normal: btPlaneSpace1 in world axes, then into base coordinates
             const V3 n = nworld;
             V3 t1, t2;
             if (fabsf(n.z) > 0.70710678118654752f) {
@@ -1459,7 +1461,7 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
     // read the joints, and without this a robot with a NaN joint angle would step on with its NaN state
     bad = bad || !(fabsf(qd[0]) <= P.vmax) || !(fabsf(ww.x) <= P.vmax) || !(fabsf(vw.x) <= P.vmax) || !isfinite(q[0] + q[1] + q[2]);
     // ---------------- mocap clock (PLE:208-210): sampled with the time *before* the increment
-    if (ENV == 0 && sub == P.substeps - 1) {
+    if (ENV == kPmc && sub == P.substeps - 1) {
       frame_id = (int)floor(time / P.frame_dt);
       frame_frac = (time - frame_id * P.frame_dt) / P.frame_dt;
       const int last = mc.clip_off[clip + 1] - mc.clip_off[clip] - P.margin + 2;     // see llq_kernels.cuh: runaway cursors only
@@ -1505,9 +1507,9 @@ __global__ void __launch_bounds__(LLQ16_BLOCK, LLQ16_MINB * 128 / LLQ16_BLOCK) l
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) { cr += __shfl_xor_sync(FULL, cr, o); lr += __shfl_xor_sync(FULL, lr, o); ov += __shfl_xor_sync(FULL, ov, o); }
     if ((threadIdx.x & 31) == 0) {
-      if (cr) atomicAdd(&E.counters[2], (unsigned long long)cr);
-      if (lr) atomicAdd(&E.counters[3], (unsigned long long)lr);
-      if (ov) atomicAdd(&E.counters[5], (unsigned long long)ov);
+      if (cr) atomicAdd(&E.counters[LLQ_CNT_CONTACT_ROWS], (unsigned long long)cr);
+      if (lr) atomicAdd(&E.counters[LLQ_CNT_LIMIT_ROWS], (unsigned long long)lr);
+      if (ov) atomicAdd(&E.counters[LLQ_CNT_DROPPED], (unsigned long long)ov);
     }
   }
   __pipeline_wait_prior(0);                                // this thread's share of the history prefetch has landed

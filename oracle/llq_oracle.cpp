@@ -582,7 +582,7 @@ bool physics_substep(llq_engine& E, Env& e, const double* tau, int64_t* n_contac
   if (nc > LLQ_MAX_CONTACTS) {
     const int64_t dropped = nc - LLQ_MAX_CONTACTS;
 #pragma omp atomic
-    E.counters[5] += dropped;
+    E.counters[LLQ_CNT_DROPPED] += dropped;
     nc = LLQ_MAX_CONTACTS;
   }
   // (b) joint damping (pybullet applyJointDamping) + motor torque, forward dynamics, velocity prediction
@@ -627,7 +627,7 @@ bool physics_substep(llq_engine& E, Env& e, const double* tau, int64_t* n_contac
       if ((int)lim.size() < LLQ_MAX_LIMIT_ROWS) lim.push_back(r);
       else {
 #pragma omp atomic
-        E.counters[5] += 1;
+        E.counters[LLQ_CNT_DROPPED] += 1;
       }
     }
   }
@@ -1797,7 +1797,7 @@ int llq_step_ex(llq_handle h, const float* actions, float* obs, int64_t obs_ld, 
       Env& e = h->envs[i];
       if (!epmc) h->avg_reward[e.clip] = e.reward_sum / h->max_steps[e.clip];
       any = true;
-      h->counters[1]++;
+      h->counters[LLQ_CNT_EPISODES]++;
     }
   if (any && !epmc) update_sampling(*h);
   for (int i = 0; i < n; i++) {
@@ -1813,7 +1813,7 @@ int llq_step_ex(llq_handle h, const float* actions, float* obs, int64_t obs_ld, 
       }
   if (obs)
     for (int i = 0; i < n; i++) std::memcpy(obs + (size_t)i * obs_ld, h->envs[i].obs, sizeof(float) * od);
-  h->counters[0] += n; h->counters[2] += ncr; h->counters[3] += nlr;
+  h->counters[LLQ_CNT_ENV_STEPS] += n; h->counters[LLQ_CNT_CONTACT_ROWS] += ncr; h->counters[LLQ_CNT_LIMIT_ROWS] += nlr;
   return LLQ_OK;
 }
 

@@ -117,10 +117,10 @@ def test_heavy_ctas_match_the_oracle(built, blob, small_mocap, oracle_lib):
             c_.set(capi.F_STATE, st); c_.set(capi.F_WARMSTART, np.zeros((n, 32), np.float32))      # a fresh heap every step
             for f in (capi.F_STATE, capi.F_WARMSTART, capi.F_OBS, capi.F_TIME, capi.F_CLIP):
                 g_.set(f, c_.get(f))
-            g0, k0_ = g_.counters()[5], c_.counters()[5]
+            g0, k0_ = g_.counters()[capi.CNT_DROPPED], c_.counters()[capi.CNT_DROPPED]
             g_.step(a); c_.step(a)
             if g_ is gpu1:
-                assert g_.counters()[5] - g0 == c_.counters()[5] - k0_ == dropped, "rows beyond the caps are counted, not solved"
+                assert g_.counters()[capi.CNT_DROPPED] - g0 == c_.counters()[capi.CNT_DROPPED] - k0_ == dropped, "rows beyond the caps are counted, not solved"
         e = blockrel(gpu.get(capi.F_STATE), cpu.get(capi.F_STATE))
         m = cpu.get(capi.F_DECISION_MARGIN)
         good = (e < 1e-4) | (m < 5e-4)

@@ -27,8 +27,8 @@ def test_both_libraries_export_every_declared_symbol(built):
 
 def test_field_ids_and_aux_slots_match_header():
     txt = open(os.path.join(ROOT, "include", "llq.h")).read()
-    defs = re.findall(r"^#define LLQ_((?:F|AUX)_\w+)\s+(\d+)", txt, re.M)
-    assert len(defs) >= 16 + 25
+    defs = re.findall(r"^#define LLQ_((?:F|AUX|CNT)_\w+)\s+(\d+)", txt, re.M)
+    assert len(defs) >= 16 + 25 + 6
     for name, value in defs:
         assert getattr(capi, name) == int(value), name
 
@@ -79,7 +79,7 @@ def test_state_roundtrip_and_counters(make_oracle):
     assert np.array_equal(eng.get(capi.F_STATE), st)
     o, r, d = eng.step(np.zeros((5, 12), np.float32))
     assert o.shape == (5, 207) and r.shape == (5,) and d.dtype == np.uint8
-    assert eng.counters()[0] == 5
+    assert eng.counters()[capi.CNT_ENV_STEPS] == 5
     assert np.all(eng.get(capi.F_EPISODE_STEPS) == 1)
 
 

@@ -26,7 +26,7 @@ def test_energy_and_momentum_conservation(model, make_oracle):
         m0 = mechanics(model, st)
         s1 = _run(eng, st, int(round(0.1 / dt)))
         m1 = mechanics(model, s1)
-        assert eng.counters()[3] == 0, "state must stay inside the joint limits for this test"
+        assert eng.counters()[capi.CNT_LIMIT_ROWS] == 0, "state must stay inside the joint limits for this test"
         drift.append((abs(m1["KE"] - m0["KE"]) / m0["KE"], np.abs(m1["P"] - m0["P"]).max(), np.abs(m1["L"] - m0["L"]).max()))
     assert drift[0][0] < 2e-5 and drift[0][1] < 1e-4 and drift[0][2] < 3e-4
     # first-order integrator: errors shrink ~4x when dt shrinks 4x
@@ -87,9 +87,9 @@ def test_contact_needs_proximity(make_oracle):
     eng.reset_to(0, 0.1)
     st = eng.get(capi.F_STATE); st[0, 2] += 1.0
     eng.set(capi.F_STATE, st)
-    c0 = eng.counters()[2]
+    c0 = eng.counters()[capi.CNT_CONTACT_ROWS]
     eng.step(np.zeros((1, 12), np.float32))
-    assert eng.counters()[2] == c0
+    assert eng.counters()[capi.CNT_CONTACT_ROWS] == c0
     assert np.all(eng.get(capi.F_WARMSTART) == 0)
 
 

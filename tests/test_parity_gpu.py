@@ -214,4 +214,4 @@ def test_ragged_batch_sizes(n, make_cuda, make_oracle):
         ok = (dc == 0) & (dg == 0) & ~near                      # finished envs were re-seeded by each side's own table
         e = np.maximum(blockrel(og[:, :99], oc[:, :99]), blockrel(og[:, 135:], oc[:, 135:]))
         assert np.all(e[ok] < TOL) and np.all(np.abs(rg - rc)[ok] < TOL)
-    assert gpu.counters()[0] == 4 * n
+    assert gpu.counters()[capi.CNT_ENV_STEPS] == 4 * n

@@ -47,12 +47,12 @@ def main():
             for _ in range(a.warmup):
                 e.step(act)
             ms = []
-            c0 = e.counters()[1]
+            c0 = e.counters()[capi.CNT_EPISODES]
             for _ in range(a.steps):
                 e.step(act)
                 e.sync()
                 ms.append(e.timing()[1])
-            resets = int(e.counters()[1] - c0)
+            resets = int(e.counters()[capi.CNT_EPISODES] - c0)
             res[C].append(dict(reset_ms=float(np.mean(ms)), resets_per_step=resets / a.steps))
             print(json.dumps(dict(round=r, clips=C, reset_ms_mean=round(float(np.mean(ms)), 5), reset_ms_median=round(float(np.median(ms)), 5),
                                   resets_per_step=round(resets / a.steps, 1))), flush=True)

@@ -68,7 +68,7 @@ def dump(lib_path, out, steps=300):
             if f in (capi.F_SAMPLE_PROB, capi.F_AVG_REWARD) and eng.n_clips == 0:
                 continue
             arrays["%s/field%d" % (name, f)] = eng.get(f)
-        print("%-12s episodes finished %d" % (name, int(eng.counters()[1])))
+        print("%-12s episodes finished %d" % (name, int(eng.counters()[capi.CNT_EPISODES])))
         eng.close()
     np.savez_compressed(out, **arrays)
 

@@ -36,7 +36,7 @@ for n in (5, 70):
     e.reset()
     for t in range(25):
         e.step((1.0 * rng.standard_normal((n, 12))).astype(np.float32))
-    assert e.counters()[5] == 0
+    assert e.counters()[capi.CNT_DROPPED] == 0
     e.close()
     from lifelike_agility_and_play_b200.sim_envs.chase_tag_game_env import sepmc_engine_config
     n2 = n + (n & 1)
