@@ -178,6 +178,16 @@ int llq_hier_policy_set_pool_model(llq_hier_policy_handle h, int32_t k, const fl
                                    void* stream);
 const char* llq_hier_policy_last_error(void);
 
+/* ---- the learner seat of a strategic-level trajectory slab (csrc/llq_seat_pack.cu), for the hand-over of unrolls to the learner rank:
+ * d_out [steps, pairs, 984] = the seat-0 rows d_slab[t, 2p] of a [steps, 2 pairs, 984] fp32 slab (row 2p of a step is the learning robot
+ * of pair p, row 2p + 1 its opponent), a bit-exact copy in 16-byte vectors; both contiguous.  Asynchronous on `stream` (0 = the default
+ * stream) of the pointers' device.  LLQ_EINVAL before the device is touched: a null pointer, a pointer that is not 16-byte aligned,
+ * steps or pairs < 1 or too large for one launch, an output overlapping the slab; then LLQ_EINVAL for pointers that are not device
+ * memory of one device.  Message via llq_seat_pack_last_error(). */
+#define LLQ_SEPMC_RECORD 984
+int llq_seat_pack(const float* d_slab, float* d_out, int64_t steps, int64_t pairs, void* stream);
+const char* llq_seat_pack_last_error(void);
+
 #ifdef __cplusplus
 }
 #endif

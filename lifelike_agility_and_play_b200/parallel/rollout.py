@@ -30,16 +30,18 @@ they take effect from the next `step()`, and the LSTM states, masks, counters an
 with the new weights.
 Several GPUs: `UnrollExchange(worker)` hands each finished unroll to the learner rank in place (the slab and the per-slab state, mask and
 bootstrap value go out of the worker's own buffers in one NCCL group); the worker's stream waits on the device for a slab's hand-over
-before it writes into that slab again.
+before it writes into that slab again.  At the strategic level `learner_seat_only=True` sends the seat-0 records alone, packed into a
+contiguous buffer first (`pack_learner_seat`), half the bytes.
 The recurrent levels keep their LSTM states on the device ([N, 128] at the environmental level: code LSTM, then value LSTM; [P, 192]
 for seat 0 at the strategic level: heading, code and value LSTM, and [P, 128] for seat 1), and each forward receives the done flags of
 the step before it, so a finished episode's state is wiped exactly where the reference actor's mask is set.
 """
+import ctypes as C
 from collections import namedtuple
 
 import torch
 
-from ..policy_epmc import DeviceHierPolicy, DeviceOpponentPool, DeviceSepmcTrainPolicy
+from ..policy_epmc import DeviceHierPolicy, DeviceOpponentPool, DeviceSepmcTrainPolicy, _policy_lib
 from .trajectory import (ACT_DIM, COL_NEGLOGP, COL_VALUE, HCOL_CODE, HCOL_NEGLOGP, HCOL_VALUE, HIER_OBS_DIM, HIER_TRAJ_WIDTH, OBS_DIM,
                          SCOL_CODE, SCOL_HEADING, SCOL_NEGLOGP, SCOL_OPPONENT, SCOL_VALUE, SEPMC_OBS_DIM, SEPMC_TRAJ_WIDTH, TRAJ_WIDTH, HandOver)
 
@@ -47,6 +49,29 @@ from .trajectory import (ACT_DIM, COL_NEGLOGP, COL_VALUE, HCOL_CODE, HCOL_NEGLOG
 # mask [rows] (uint8) its first forward started from, and V(observation T) [rows]; all valid until the end of the NEXT unroll
 Unroll = namedtuple("Unroll", ["slab", "initial_state", "first_mask", "bootstrap_value"])
 _FSZ = 4                                    # bytes per float: column offsets into a slab row
+_seat_lib = None
+
+
+def pack_learner_seat(slab, out, stream=None):
+    """`out` [T, P, 984] = `slab[:, 0::2]` of a strategic-level `[T, 2P, 984]` slab, the learning robots' records, bit for bit, by the
+    pack kernel (include/llq_policy.h, llq_seat_pack); both contiguous float32 on one CUDA device.  Asynchronous on `stream` (a
+    torch.cuda.Stream; default: the current stream)."""
+    global _seat_lib
+    W = SEPMC_TRAJ_WIDTH
+    if not (isinstance(slab, torch.Tensor) and isinstance(out, torch.Tensor) and slab.dim() == 3 and out.dim() == 3 and out.shape[2] == W
+            and tuple(slab.shape) == (out.shape[0], 2 * out.shape[1], W) and slab.dtype == out.dtype == torch.float32
+            and slab.is_cuda and slab.device == out.device and slab.is_contiguous() and out.is_contiguous()):
+        raise ValueError("pack_learner_seat takes a contiguous float32 [T, 2P, %d] slab and a [T, P, %d] output on one CUDA device, got %s %s"
+                         % (W, W, getattr(slab, "shape", slab), getattr(out, "shape", out)))
+    T, P = out.shape[:2]
+    if _seat_lib is None:
+        lib = _policy_lib()
+        lib.llq_seat_pack.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]
+        lib.llq_seat_pack_last_error.restype = C.c_char_p
+        _seat_lib = lib
+    s = torch.cuda.current_stream(out.device) if stream is None else stream
+    if _seat_lib.llq_seat_pack(slab.data_ptr(), out.data_ptr(), T, P, s.cuda_stream):
+        raise RuntimeError("llq_seat_pack: %s" % _seat_lib.llq_seat_pack_last_error().decode())
 
 
 class _SlabWorker:
@@ -327,27 +352,41 @@ class UnrollExchange:
     ranks.  A world of 1 returns the worker's own views, with no copy (`own_copy=True` copies them as a learner rank of a larger world
     copies its own unroll).
 
-    The strategic level sends the slab as the worker wrote it, both seats: the opponent's model (column 983) travels in the seat-0
-    records, and the seat-1 records double the bytes (4.13 GB per rank and unroll at T = 128, P = 4096, half of it seat 1).
+    The strategic level sends by default the slab as the worker wrote it, both seats: the opponent's model (column 983) travels in the
+    seat-0 records, and the seat-1 records, which the learner never reads, double the bytes (4.13 GB per rank and unroll at T = 128,
+    P = 4096).  `learner_seat_only=True` (a `SepmcRolloutWorker` only) sends the seat-0 records alone: `hand_over` first packs them into
+    one contiguous `[T, P, 984]` send buffer of the exchange (`pack_learner_seat`, on the side stream behind the worker's stream and
+    behind the previous transfer out of that buffer), then sends that buffer in the slab's place, with the same state, mask and bootstrap
+    value.  The slab's hand-over event is recorded behind the pack and the transfer, so the worker rewrites a slab only after both.
+    `gathered(b)` returns `Unroll(slab [T, P, 984], initial_state, first_mask, bootstrap_value)` per rank, for
+    `sepmc_slab_records(..., learner_seat_only=True)`; a world of 1 without `own_copy` returns the send buffer itself, which the next
+    `hand_over` packs again once the next unroll is complete: valid, like the worker's views, until the end of the next unroll.
+    `bytes_per_rank` is 2.07 GB at T = 128, P = 4096, and every rank keeps one send buffer of 2.06 GB.  One buffer is enough: the
+    next pack waits for the worker's whole next unroll, which takes far longer than a transfer.
 
     Memory on the learner rank: `2 x world x bytes_per_rank` bytes of receive buffers, `bytes_per_rank` = T*N*W*4 + state + mask +
     bootstrap, on top of the worker's own two `[T+1, N, W]` slabs.  At T = 128: PMC at N = 4096 sends 0.47 GB per rank (7.5 GB for
     8 ranks); EPMC at N = 8192 3.93 GB (62.9 GB for 8 ranks, plus 7.9 GB of slabs: too much next to an engine on an 80 GB card), at
     N = 4096 1.97 GB (31.4 GB for 8 ranks, plus 4.0 GB of slabs: fits on an 80 GB learner rank); SEPMC at P = 4096 4.13 GB (66.1 GB for
-    8 ranks).
+    8 ranks), or with `learner_seat_only` 2.07 GB (33.1 GB for 8 ranks, plus 8.3 GB of slabs and the 2.06 GB send buffer).
     """
 
-    def __init__(self, worker, dst=0, group=None, own_copy=None):
+    def __init__(self, worker, dst=0, group=None, own_copy=None, learner_seat_only=False):
         if not isinstance(worker, _SlabWorker):
             raise ValueError("UnrollExchange hands over the unrolls of a RolloutWorker, HierRolloutWorker or SepmcRolloutWorker")
+        self.learner_seat_only = bool(learner_seat_only)
+        if self.learner_seat_only and not isinstance(worker, SepmcRolloutWorker):
+            raise ValueError("learner_seat_only is for a SepmcRolloutWorker: the other levels have one seat")
         self.worker = worker
         self.recurrent = isinstance(worker, _RecurrentWorker)
+        self.send = worker._zeros(worker.T, worker.rows, SEPMC_TRAJ_WIDTH) if self.learner_seat_only else None
         self.core = HandOver([(x.shape, x.dtype) for x in self._tensors(0)], worker.dev, dst, group, own_copy)
         self.world, self.rank, self.dst, self.bytes_per_rank = self.core.world, self.core.rank, self.core.dst, self.core.bytes_per_rank
+        self._last = None                   # the ping-pong index of the last hand-over: its transfer reads the send buffer
 
     def _tensors(self, i):
         w = self.worker
-        slab = w.bufs[i][:w.T]
+        slab = self.send if self.learner_seat_only else w.bufs[i][:w.T]
         return (slab, w.init_states[i], w.first_masks[i], w.boots[i]) if self.recurrent else (slab, w.boots[i])
 
     def hand_over(self, u):
@@ -358,8 +397,16 @@ class UnrollExchange:
         i = next((k for k in (0, 1) if slab.data_ptr() == w.bufs[k].data_ptr()), None)
         if i is None or i == w._slab_index():
             raise ValueError("hand_over() takes the unroll the worker's finish_unroll() returned last")
-        self.core.post(i, self._tensors(i), stream=w.stream)
-        w.handed[i] = self.core.sent[i]
+        stream = w.stream
+        if self.learner_seat_only:
+            stream = self.core.side
+            stream.wait_stream(w.stream)
+            if self._last is not None:
+                stream.wait_event(self.core.sent[self._last])      # the previous transfer has left the send buffer
+            pack_learner_seat(slab, self.send, stream)
+        self.core.post(i, self._tensors(i), stream=stream)
+        w.handed[i] = self.core.sent[i]     # recorded behind the pack and the transfer: the worker rewrites slab i after both
+        self._last = i
         return i
 
     def gathered(self, b):

@@ -120,17 +120,25 @@ SEPMC_OBS_LEAVES = OrderedDict([("prop", (99,)), ("prop_a", (36,)), ("percept_2d
                                 ("flag_info_cheat", (7,)), ("with_flag", (2,)), ("control_spd", (1,))])
 
 
-def sepmc_slab_records(slab, initial_state, first_mask, bootstrap_value, gamma=GAMMA, lam=LAM, with_opponent=False):
+def sepmc_slab_records(slab, initial_state, first_mask, bootstrap_value, gamma=GAMMA, lam=LAM, with_opponent=False, learner_seat_only=False):
     """Learner tensors of a strategic-level unroll (`SepmcRolloutWorker.finish_unroll()`) for the learning robot (seat 0: rows 0, 2, 4, ...
     of the `[T, 2P, 984]` slab), on the slab's device, named: the twelve observation leaves [T, P, *leaf] (CTG:111-124), `A_HLC` [T, P]
     (the raw sampled heading), `A_Z` [T, P] int64 (the argmax code), `neglogp` (of the heading), `discount` = gamma (1 - done), `r`, `V`,
     `R` (lambda-returns, bootstrapped with V(observation T)), `M` [T, P] = the mask each forward received (M[0] = first_mask, M[t] =
     done[t-1]) -- all [T, P] float32 but A_Z -- and `S` [P, 192], the recurrent state the unroll started from (heading, code and value
     LSTM, [c, h] each).  `with_opponent`: also `opponent` [T, P] int64 last, the index of the model seat 1 played in an opponent
-    pool (for the league's per-opponent statistics; 0 against a single opponent)."""
-    assert slab.dim() == 3 and slab.shape[2] == SEPMC_TRAJ_WIDTH and slab.shape[1] % 2 == 0, \
-        "expected a [T, 2P, %d] trajectory slab" % SEPMC_TRAJ_WIDTH
-    s0 = slab[:, 0::2]
+    pool (for the league's per-opponent statistics; 0 against a single opponent).  `learner_seat_only`: `slab` holds the seat-0 records
+    alone, `[T, P, 984]` (what `UnrollExchange(..., learner_seat_only=True)` gathers); the tensors are those of the full slab, bit for bit.
+    P is the length of `first_mask`."""
+    P = first_mask.shape[0]
+    if learner_seat_only:
+        assert slab.dim() == 3 and slab.shape[2] == SEPMC_TRAJ_WIDTH and slab.shape[1] == P, \
+            "expected a [T, P, %d] learner-seat slab (P = len(first_mask) = %d)" % (SEPMC_TRAJ_WIDTH, P)
+        s0 = slab
+    else:
+        assert slab.dim() == 3 and slab.shape[2] == SEPMC_TRAJ_WIDTH and slab.shape[1] == 2 * P, \
+            "expected a [T, 2P, %d] trajectory slab (P = len(first_mask) = %d)" % (SEPMC_TRAJ_WIDTH, P)
+        s0 = slab[:, 0::2]
     out = _recurrent_records(s0, SEPMC_OBS_LEAVES, [("A_HLC", s0[:, :, SCOL_HEADING]), ("A_Z", s0[:, :, SCOL_CODE].to(torch.int64))],
                              (SCOL_NEGLOGP, SCOL_REWARD, SCOL_DONE, SCOL_VALUE), initial_state, first_mask, bootstrap_value, gamma, lam)
     if with_opponent:

@@ -74,7 +74,8 @@ POLICY_EXPORTS = ["llq_policy_create", "llq_policy_destroy", "llq_policy_forward
                   "llq_policy_last_error", "llq_hier_policy_create", "llq_hier_policy_destroy", "llq_hier_policy_forward",
                   "llq_hier_policy_last_error", "llq_hier_policy_create_train", "llq_hier_policy_forward_rec",
                   "llq_hier_policy_create_pool", "llq_hier_policy_set_pool_probs", "llq_hier_policy_forward_pool",
-                  "llq_policy_set_weights", "llq_hier_policy_set_weights", "llq_hier_policy_set_pool_model"]
+                  "llq_policy_set_weights", "llq_hier_policy_set_weights", "llq_hier_policy_set_pool_model", "llq_seat_pack",
+                  "llq_seat_pack_last_error"]
 N_WEIGHTS = 358647
 # array shapes of a shipped primitive-level *.model file, in their stored order (the 28 arrays of include/llq_policy.h)
 PMC_SHAPES = [(1, 135), (1, 135), (1, 72), (1, 72), (207, 256), (256,), (256, 256), (256,), (256, 1), (1,), (207, 256), (256,), (256, 256),
