@@ -92,8 +92,8 @@ void fill_params(llq_handle h) {
   P.ph_lo = (float)c.push_h_lo; P.ph_hi = (float)c.push_h_hi; P.pv_lo = (float)c.push_v_lo; P.pv_hi = (float)c.push_v_hi;
   P.ts_lo = (float)c.target_spd_lo; P.ts_hi = (float)c.target_spd_hi;
   P.knee = c.knee_contacts; P.mu_wheel = (float)(c.ground_friction * c.link_friction); P.aux_r = (float)c.auxiliary_radius;
-  P.element_id = c.element_id; P.ww_lo = (float)c.wall_width_lo; P.ww_hi = (float)c.wall_width_hi; P.wg_lo = (float)c.wall_gap_lo;
-  P.wg_hi = (float)c.wall_gap_hi; P.hg_lo = (float)c.hole_gap_lo; P.hg_hi = (float)c.hole_gap_hi;
+  P.element_id = c.element_id; P.ww_lo = c.wall_width_lo; P.ww_hi = c.wall_width_hi; P.wg_lo = c.wall_gap_lo;
+  P.wg_hi = c.wall_gap_hi; P.hg_lo = c.hole_gap_lo; P.hg_hi = c.hole_gap_hi;
   if (!h->has_obstacles) { P.has_ob = 0; P.ob_hx = P.ob_hy = P.ob_hz = 0.f; }
 }
 

@@ -95,10 +95,13 @@ struct StepParams {
   // PMC hurdle plates (PLE:173-193)
   int has_ob; float ob_hx, ob_hy, ob_hz;
   // EPMC corridor (BSE)
-  int element_id; float ww_lo, ww_hi, wg_lo, wg_hi, hg_lo, hg_hi;
+  int element_id;
   // knee-wheel ground contact (llq_config.knee_contacts / link_friction)
   int knee; float mu_wheel;
   float aux_r;      // EPMC elements 1-3: radius of the auxiliary edge cylinders (0 = none)
+  // EPMC corridor terrain ranges (wall width, wall gap, hole gap): double, as the reference draws them (BSE:171-174, 372-373); an
+  // fp32 bound such as 0.3 moves a bar centre by one fp32 ulp in a fifth of the draws.  The step kernel does not read them.
+  double ww_lo, ww_hi, wg_lo, wg_hi, hg_lo, hg_hi;
 };
 
 struct EnvArrays {      // SoA device arrays, N envs
@@ -499,7 +502,7 @@ LLQ_DI void put_box(float* boxes, int& nb, bool wr, double cx, double cy, double
 LLQ_DI int generate_corridor(const StepParams& P, unsigned long long seed, long long gid, long long ep, float* boxes, bool wr, double& tgx) {
   TerrainRng R{seed, gid, ep, 0, {0.0, 0.0, 0.0, 0.0}};
   int nb = 0;
-  const double width = R.uniform((double)P.ww_lo, (double)P.ww_hi), gap = R.uniform((double)P.wg_lo, (double)P.wg_hi);
+  const double width = R.uniform(P.ww_lo, P.ww_hi), gap = R.uniform(P.wg_lo, P.wg_hi);
   put_box(boxes, nb, wr, 5.0, gap / 2.0 + width / 2.0, 1.0, 200.0, width, 2.0);
   put_box(boxes, nb, wr, 5.0, -(gap / 2.0 + width / 2.0), 1.0, 200.0, width, 2.0);
   double cur = 0.0;
@@ -513,7 +516,7 @@ LLQ_DI int generate_corridor(const StepParams& P, unsigned long long seed, long 
           put_box(boxes, nb, wr, cur + d / 2, 0.0, h / 2, 0.1, gap, h);
           cur += d + 0.1;
         } else {
-          const double d = R.uniform(1.0, 3.0), g = R.uniform((double)P.hg_lo, (double)P.hg_hi);
+          const double d = R.uniform(1.0, 3.0), g = R.uniform(P.hg_lo, P.hg_hi);
           put_box(boxes, nb, wr, cur + d / 2, 0.0, 0.3 / 2 + g, 0.1, gap, 0.3);
           cur += d + 0.1;
         }
